@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — KV-block offload throughput (save + load) on N x B200, one process per GPU.
+"""bench.py — KV-block offload throughput (save + load) on N x H100, one process per GPU.
 
 Metric (BASELINE.json): KV-block offload GB/s (save+load); blocks/sec.
 Workload at N=1 = BASELINE config #2: Llama-3-8B fp16 paged KV, 16-token blocks
@@ -55,6 +55,7 @@ MIGRATE_BLOCKS = 2048                          # BASELINE config #4: 32k-token c
 # bounded so that the whole --steps K --warmup W run stays within a few minutes.  The full 10 000 blocks when the run is
 # short enough, never fewer than 2048, and the number REALLY used is what `config.blocks_per_step` reports.
 FILE_TIER_BLOCK_BUDGET = 100_000               # blocks moved each way over the whole run, per rank
+HBM_DATASHEET_GBS = bx.HBM_DATASHEET_GBS
 
 
 def file_tier_blocks(steps: int, warmup: int) -> int:
@@ -89,7 +90,7 @@ def env_int(name, d):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region."""
 
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -135,7 +136,7 @@ def measured_hbm_peak():
     try:
         return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+        return HBM_DATASHEET_GBS, "fallback (H100 SXM data sheet, 3.35 TB/s)"
 
 
 def load_reference_engine():
@@ -246,6 +247,30 @@ def single_file_job_latency(eng, ids, root, jobs=40, first_job=500000, cleanup=N
             "blocks_per_job": bpf, "bytes_per_job": bpf * BLOCK_BYTES, "jobs": len(st)}
 
 
+def _row_sums(rows):
+    """Byte sums of the rows of a uint8 (R, frag) tensor, exact in int32, in slices that keep the widened copy small."""
+    import torch
+    return torch.cat([rows[i:i + 8192].to(torch.int32).sum(dim=1) for i in range(0, rows.shape[0], 8192)])
+
+
+def dump_outputs(out_dir, big, ids_dev, packed) -> None:
+    """What the last timed step handed its callers, as .npy files (about 26 MB): the gather's packed buffer and the pool
+    the scatter wrote back.  Every fragment is covered by its byte sum (exact in float64); the same fixed, seeded sample
+    of single bytes (float32) from both catches errors that leave a sum unchanged."""
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    T, n_blocks, frag = big.shape[0], ids_dev.numel(), big.shape[2]
+    out = {"block_ids": ids_dev.cpu().numpy(),
+           "packed_fragment_sums": _row_sums(packed.view(n_blocks * T, frag)).view(n_blocks, T).cpu().numpy(),
+           "pool_fragment_sums": torch.stack([_row_sums(big[t, ids_dev]) for t in range(T)], dim=1).cpu().numpy()}
+    g = torch.Generator(device=packed.device).manual_seed(2024)
+    pos = torch.randint(0, packed.numel(), (1 << 21,), device=packed.device, generator=g)
+    out["packed_byte_sample"] = packed[pos].cpu().numpy()
+    out["pool_byte_sample"] = big[(pos // frag) % T, ids_dev[pos // (T * frag)], pos % frag].cpu().numpy()
+    for name, a in out.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a.astype(np.float32 if a.dtype == np.uint8 else np.float64))
+
+
 def pool_checksum(big) -> int:
     """64-bit wrap-around sum of every 8-byte word of the pool (order independent)."""
     import torch
@@ -271,7 +296,7 @@ def workload_config(n_gpus, blocks_per_step=N_BLOCKS):
            "blocks_per_step": blocks_per_step, "workload_blocks": N_BLOCKS,
            "block_ids": f"rng(1).permutation({POOL_BLOCKS})[:{blocks_per_step}] (non-contiguous, unsorted)",
            "gpu_blocks_per_file": BLOCKS_PER_FILE, "partitioning": f"{n_gpus} independent KV partitions (one per GPU)",
-           "l2_policy": f"inputs_exceed_l2 ({blocks_per_step * BLOCK_BYTES / 1e9:.2f} GB per pass vs 126 MB L2)"}
+           "l2_policy": f"inputs_exceed_l2 ({blocks_per_step * BLOCK_BYTES / 1e9:.2f} GB per pass vs 50 MB L2)"}
     return cfg
 
 
@@ -482,6 +507,8 @@ def run_ours(args):
     dev_ms = max_over_ranks(dist, start.elapsed_time(stop))
     gather_ms = float(np.mean([e[0].elapsed_time(e[1]) for e in ev_sets]))
     scatter_ms = float(np.mean([e[1].elapsed_time(e[2]) for e in ev_sets]))
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, big, ids_dev, packed)
     # untimed proof that the load leg really restores: save, ZERO every saved page, load, compare
     sum0 = pool_checksum(big)
     pool.gather_dev(ids_dev, packed)
@@ -616,6 +643,7 @@ def run_ours(args):
         tot_t = max_over_ranks(dist, time.perf_counter() - tt0)
         pg = bx.gather_objects(dist, {"store": payload * 2 / st_t / 1e9, "load": payload * 2 / max(mine_t - st_t, 1e-9) / 1e9})
         eng_t.shutdown()
+        del eng_t
         assert pool_checksum(big) == sum0, "huge-page arena save+load did not restore the pool bit-exact"
         thp_arm = {"value": world * 2 * payload * 2 / tot_t / 1e9, "unit": "GB/s", "steps": 2,
                    "store_gbs_per_gpu": [round(x["store"], 2) for x in pg], "load_gbs_per_gpu": [round(x["load"], 2) for x in pg],
@@ -648,7 +676,9 @@ def run_ours(args):
 
     # ---- extras on their own data: config #3 (every rank, weak scaling), then configs #1 / #5 / ingest (rank 0)
     pool.close()
-    del check_ref, tensors, big, ids_dev
+    # the engines hold the pool (and through it this workload's 26 GB of tensors): drop every reference before config #3
+    # allocates its own pool and packed buffer, or the two workloads would not fit 80 GB together
+    del check_ref, check_ids, tensors, big, ids_dev, pool, eng, eng_d
     torch.cuda.empty_cache()
     if not args.no_extras:
         c3 = bx.run_config3(kvb, dist, rank, world, local, args.steps, args.warmup, peak, peak_src,
@@ -697,7 +727,7 @@ def run_ours(args):
                          "unit": "GB/s", "frac": achieved / peak, "traffic": traffic, "peak_source": peak_src,
                          "algorithmic_bytes_per_launch": 2 * payload, "gather_ms": gather_ms, "scatter_ms": scatter_ms,
                          "scatter_achieved": 2 * payload / (scatter_ms / 1e3) / 1e9,
-                         "frac_of_nominal_8TBs": achieved / 8000.0},
+                         "frac_of_datasheet": achieved / HBM_DATASHEET_GBS},
             "clocks": clocks,
         }
         if cpu_baseline is not None:
@@ -809,8 +839,12 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-migration", action="store_true")
     ap.add_argument("--no-extras", action="store_true", help="skip configs #1/#3/#5, ingest and manager lookup (ncu captures)")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="after the timed steps, write what the last one computed (packed "
+                    "buffer and restored pool: per-fragment byte sums and a seeded byte sample) as DIR/<name>.npy")
     args = ap.parse_args()
     if args.impl == "reference":
+        if args.dump_outputs:  # the reference arm moves files through its own engine and hands no buffer back
+            ap.error("--dump-outputs applies to the default arm (--impl ours) only")
         return run_reference(args)
     return run_ours(args)
 

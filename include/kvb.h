@@ -1,4 +1,4 @@
-/* kvb.h — C ABI of libkvb.so, the B200-native (sm_100a) KV-block hot path.
+/* kvb.h — C ABI of libkvb.so, the H100-native (sm_90a) KV-block hot path.
  *
  * This is the drop-in boundary: plain pointers and sizes, no torch / C++ types.
  * Each group of entry points names the reference interface it replaces
@@ -13,10 +13,10 @@
  *   - "stream" arguments are cudaStream_t passed as void*; NULL = legacy default stream.
  *   - block ids are int64 (reference: std::vector<int64_t>, storage_offload.hpp:104-109).
  *   - there is NO CPU fallback: every compute entry point fails with KVB_ERR_CUDA
- *     when no sm_100 device is usable.
+ *     when no sm_90 device is usable.
  *   - environment switches (diagnostics and A/B runs, never needed for correctness):
  *       KVB_HASH_KERNEL=lanes   hash with the lane-per-prompt kernels at every batch size (read per call)
- *       KVB_HASH_KERNEL=wpc     hash with the warp-per-prompt kernel at every batch size it supports (the default up to 1536 prompts)
+ *       KVB_HASH_KERNEL=wpc     hash with the warp-per-prompt kernel at every batch size it supports (the default up to 10 prompts per SM: 1320 on an H100)
  *       KVB_HASH_KERNEL=chain   hash with round 2's chain kernel in its hash-only form (it is the fused scoring launch's kernel)
  *       KVB_HASH_KERNEL=spec    the table kernel for every batch it can take (<= 64 prompts, <= 16384 keys; default: <= 32 prompts)
  *       KVB_HASH_SPEC=0         never pick the table kernel;  KVB_SPEC_SCORE_BATCH=1..32  keys its scorer warp waits for

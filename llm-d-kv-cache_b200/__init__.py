@@ -1,4 +1,4 @@
-"""llm-d-kv-cache_b200 — B200-native (sm_100a) KV-block hot path behind the reference's own surfaces.
+"""llm-d-kv-cache_b200 — H100-native (sm_90a) KV-block hot path behind the reference's own surfaces.
 
 The directory name is not a Python identifier; import it with
     kvb = importlib.import_module("llm-d-kv-cache_b200")

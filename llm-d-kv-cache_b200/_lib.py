@@ -132,7 +132,7 @@ def load() -> C.CDLL:
     if not os.path.exists(LIB_PATH):
         raise ImportError(
             f"{LIB_PATH} is missing: build it with `python llm-d-kv-cache_b200/build.py` "
-            "(nvcc, sm_100a).  There is no CPU fallback for this path.")
+            "(nvcc, sm_90a).  There is no CPU fallback for this path.")
     lib = C.CDLL(LIB_PATH, mode=C.RTLD_GLOBAL)
     bind(lib)  # AttributeError => ABI mismatch, fail loudly
     if lib.kvb_abi_version() != ABI_VERSION:

@@ -1,4 +1,4 @@
-"""Build libkvb.so (sm_100a) in-tree with nvcc.  No torch involved: the library is plain CUDA runtime + C ABI.
+"""Build libkvb.so (sm_90a) in-tree with nvcc.  No torch involved: the library is plain CUDA runtime + C ABI.
 
     python llm-d-kv-cache_b200/build.py [--force] [--verbose]
 """
@@ -16,7 +16,7 @@ LIB = os.path.join(HERE, "libkvb.so")
 OBJ = os.path.join(HERE, "build")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC,-O3,-Wall,-Wno-unused-function",
     "-I", os.path.join(ROOT, "include"), "-I", CSRC,
@@ -27,7 +27,7 @@ def _nvcc() -> str:
     for c in (os.environ.get("NVCC"), shutil.which("nvcc"), "/usr/local/cuda/bin/nvcc"):
         if c and os.path.exists(c):
             return c
-    raise RuntimeError("nvcc not found (needed to build libkvb.so for sm_100a)")
+    raise RuntimeError("nvcc not found (needed to build libkvb.so for sm_90a)")
 
 
 def sources() -> list[str]:
@@ -68,9 +68,9 @@ def build(force: bool = False, verbose: bool = False) -> str:
         failed |= p.returncode != 0
     if failed:
         raise RuntimeError("nvcc failed building libkvb.so")
-    cmd = [nvcc, "-shared", "-o", LIB + ".tmp", *objs, "-gencode", "arch=compute_100a,code=sm_100a",
+    cmd = [nvcc, "-shared", "-o", LIB + ".tmp", *objs, "-gencode", "arch=compute_90a,code=sm_90a",
            "-Xcompiler", "-fPIC", "-lpthread", "-ldl", "-lrt",
-           "-Xlinker", "--no-undefined"]  # a missing definition must fail the build, not the first dlopen on the GPU box
+           "-Xlinker", "--no-undefined"]  # a missing definition must fail the build, not the first dlopen on a GPU host
     r = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     if r.returncode != 0:
         print(r.stdout)

@@ -1,4 +1,4 @@
-// copy_kernels.cu — paged-KV gather / scatter / page->page migration kernels for sm_100a.
+// copy_kernels.cu — paged-KV gather / scatter / page->page migration kernels for sm_90a (H100).
 //
 // Replaces the reference's per-(block x tensor) cudaMemcpyAsync loop
 // (kv_connectors/llmd_fs_backend/csrc/storage/tensor_copier.cu:78-96) and its opt-in
@@ -400,8 +400,8 @@ int launch_migrate(const kvb_pool* src, const kvb_pool* dst, const int64_t* src_
   a.T = (uint32_t)src->num_tensors;
   a.total_items = (uint64_t)n * (uint64_t)src->num_tensors;
   int vec = std::min(src->vec_bytes, dst->vec_bytes);
-  // NVLink peer stores: the 16 B LDG/STG mover (unroll 4, 8 CTAs/SM) sustains more than the bulk mover
-  // (688 vs 675 GB/s per GPU in the ring sweep, profiles/r01_tune_migrate_8b_n2.log); local HBM keeps bulk
+  // NVLink peer stores default to the 16 B LDG/STG mover (unroll 4, 8 CTAs/SM): registers keep more stores in flight
+  // than the bulk ring's shared memory.  Not yet swept on H100 (tools/tune_migrate.py needs two GPUs); local HBM keeps bulk
   if ((flags & 0xff) == KVB_COPY_DEFAULT && dst->peer && vec == 16) flags = KVB_COPY_LDG | (4 << 8) | (8 << 12);
   return launch_copy<kMigrate>(a, vec, src->device, s, flags);
 }

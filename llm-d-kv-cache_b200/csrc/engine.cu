@@ -9,7 +9,7 @@
 //   * EMA-based dynamic write-queue limit that drops stores (storage_offload.cpp:80-108,272-288);
 //   * on-disk format of the CPU path: file of max(bpf*block_bytes, 16 MiB), blocks tail-aligned, written to a
 //     temp name and renamed (file_io.cpp:50-101, tensor_copier.cu:75-76).
-// What is different (B200-first):
+// What is different (GPU-first):
 //   * the unit of GPU work is a CHUNK of whole files (tens of MiB), not one (block x tensor) fragment:
 //     one gather kernel packs the chunk in HBM, ONE large pinned-async D2H moves it (the reference issues
 //     blocks x tensors cudaMemcpyAsync calls of 16-64 KiB); loads are the inverse H2D -> scatter;
@@ -32,6 +32,7 @@
 #include <condition_variable>
 #include <cstring>
 #include <deque>
+#include <future>
 #include <list>
 #include <map>
 #include <memory>
@@ -284,7 +285,7 @@ static bool read_all(int fd, uint8_t* p, int64_t n, int64_t off) {
 }
 
 // One file's payload through the page cache.  With parts > 1 the byte range is split over short-lived helper threads
-// (pread with explicit offsets is thread-safe on one descriptor): a lone 32 MiB load drops from 7.5 to 4.0 ms on tmpfs.
+// (pread with explicit offsets is thread-safe on one descriptor): a lone multi-MiB load finishes sooner on tmpfs.
 // Only reads are split — writes to ONE file serialise on the inode lock (measured: no gain) — and only when no other
 // task is queued, so the throughput regime keeps one I/O thread per worker.
 static bool file_rw(int fd, uint8_t* p, int64_t n, int64_t off, bool is_write, int parts) {
@@ -348,6 +349,7 @@ static int file_write_mode() {  // 0 = auto (mmap only for lone stores), 1 = alw
 // its own bounce buffers) — same calls, same file bytes.
 struct CuFile {
   bool ok = false;
+  bool stalled = false;  // cuFileDriverOpen did not return in kOpenWait: cuFile is never called again in this process
   CUfileError_t (*DriverOpen)() = nullptr;
   CUfileError_t (*HandleRegister)(CUfileHandle_t*, CUfileDescr_t*) = nullptr;
   void (*HandleDeregister)(CUfileHandle_t) = nullptr;
@@ -387,7 +389,19 @@ struct CuFile {
       why = "libcufile lacks a required symbol";
       return;
     }
-    const CUfileError_t st = DriverOpen();
+    // Where nvidia-fs is absent the driver open can log that it runs in compatibility mode and then not return at all
+    // (an H100 host: no answer within 400 s).  It runs on a helper thread; one that has not answered in 15 s is left
+    // behind, detached, and the engine treats the driver as stalled (DESIGN.md section 4).
+    constexpr auto kOpenWait = std::chrono::seconds(15);
+    auto done = std::make_shared<std::promise<CUfileError_t>>();
+    std::future<CUfileError_t> answer = done->get_future();
+    std::thread([done, open = DriverOpen] { done->set_value(open()); }).detach();
+    if (answer.wait_for(kOpenWait) != std::future_status::ready) {
+      why = "cuFileDriverOpen did not return within 15 s";
+      stalled = true;
+      return;
+    }
+    const CUfileError_t st = answer.get();
     if (st.err != CU_FILE_SUCCESS) {
       why = "cuFileDriverOpen failed (" + std::to_string((int)st.err) + ")";
       return;
@@ -483,7 +497,7 @@ struct kvb_engine {
   bool read_file(const FilePart& f, uint8_t* payload, int parts);
   // GDS tier: the reference's GDS file format (gds_file_io.cpp:238-418: n x block_bytes, head-aligned, tmp + rename),
   // ONE cuFile call per file between the file and the worker's packed HBM chunk
-  // When cuFile cannot register a file (observed on the GPU boxes' overlay and tmpfs mounts: CU_FILE_INTERNAL_ERROR),
+  // When cuFile cannot register a file (seen on overlay and tmpfs mounts: CU_FILE_INTERNAL_ERROR),
   // the same file format moves through the worker's pinned staging buffer instead; cufile_broken makes that sticky.
   bool gds_read = false, gds_write = false;
   std::atomic<bool> cufile_broken{false};
@@ -505,7 +519,8 @@ bool kvb_engine::worker_init(Worker& w) {
   if (opts.tier == KVB_TIER_FILE &&
       host_alloc_near(device, reinterpret_cast<void**>(&w.h_stage), chunk, cudaHostAllocDefault) != cudaSuccess)
     return false;
-  if ((gds_read || gds_write) && CuFile::get().BufRegister)  // optional: unregistered buffers go through cuFile's own
+  // optional: unregistered buffers go through cuFile's own bounce buffers
+  if ((gds_read || gds_write) && CuFile::get().ok && CuFile::get().BufRegister)
     w.packed_registered = CuFile::get().BufRegister(w.d_packed, chunk, 0).err == CU_FILE_SUCCESS;
   w.ready = true;
   return true;
@@ -1008,16 +1023,19 @@ int kvb_engine_create(kvb_pool_t* pool, const kvb_engine_opts_t* opts, kvb_engin
     }
     e->local_cpus = gpu_local_cpus(e->device);
     // KVB_FILE_SPREAD=1 (A/B, off by default): every second file-tier worker runs on the OTHER NUMA node's CPUs, so that its
-    // page-cache pages land there while its pinned staging buffer stays next to the GPU.  Measured on tmpfs
-    // (profiles/r02_file_tier_probe_b.json, 16 workers): stores 38.8 vs 36.5 GB/s, loads 29.3 vs 34.8 — the limit is the
-    // kernel's page-cache insertion path, which more threads or more nodes do not widen (24 / 32 / 48 workers are slower).
+    // page-cache pages land there while its pinned staging buffer stays next to the GPU.  On tmpfs the limit is the
+    // kernel's page-cache insertion path, which more threads or more nodes do not widen (tools/probe_file_tier.py).
     const char* spread = std::getenv("KVB_FILE_SPREAD");
     if (opts->tier == KVB_TIER_FILE && spread && spread[0] == '1') e->remote_cpus = gpu_remote_cpus(e->device);
     if (opts->tier == KVB_TIER_FILE && (opts->gds_mode & (KVB_GDS_READ | KVB_GDS_WRITE))) {
       cudaFree(nullptr);  // cuFileDriverOpen wants a CUDA context
-      if (CuFile::get().ok) {
+      if (CuFile::get().ok || CuFile::get().stalled) {
         e->gds_read = (opts->gds_mode & KVB_GDS_READ) != 0;
         e->gds_write = (opts->gds_mode & KVB_GDS_WRITE) != 0;
+        if (!CuFile::get().ok) {  // a stalled driver: the GDS file format moves through the pinned staging buffers
+          e->cufile_broken = true;
+          fprintf(stderr, "[kvb][WARN] %s: GDS-format files go through pinned staging\n", CuFile::get().why.c_str());
+        }
       } else {  // storage_offload.cpp:129-134: warn and use CPU staging for both directions
         fprintf(stderr, "[kvb][WARN] GDS requested but unavailable (%s): falling back to CPU staging\n",
                 CuFile::get().why.c_str());

@@ -11,7 +11,7 @@
 //   lane per prompt (32 chains per warp; the byte chain xor -> multiply runs serially in each lane)
 //     hash_chain_kernel_2w<BS<=16>  two warps per 32 chains: warp 0 encodes block i+1, warp 1 folds block i
 //     hash_chain_kernel<BS>         one warp does both (any block size; A/B switch KVB_HASH_ONE_WARP)
-//   warp per prompt, batches <= kWpcMaxPrompts and block size 4/8/16 (KVB_HASH_KERNEL=lanes disables it)
+//   warp per prompt, batches <= kWpcPromptsPerSm x SMs and block size 4/8/16 (KVB_HASH_KERNEL=lanes disables it)
 //     hash_chain_kernel_wpc<BS>     the 32 lanes resolve one block's byte stream together: FNV-1a is a T-function,
 //                                   so its low byte is 8 prefix-XOR rounds (warp votes) and the 64-bit state a dot
 //                                   product with powers of P^-1 (see the comment above the kernel)
@@ -45,7 +45,7 @@ __device__ __forceinline__ void fold(Fnv& h, uint32_t byte) {
   const uint32_t x = h.lo ^ byte;
   // one IMAD.WIDE gives both halves of x * 0x1b3 with a ZERO addend: written as PTX so the compiler cannot fold the
   // high-half accumulation into the wide multiply's addend, which would chain lo' behind the hi update
-  // (LOP3 -> SHL -> IMAD -> IMAD.WIDE per byte instead of LOP3 -> IMAD.WIDE; measured 33 vs ~11 cycles per byte)
+  // (LOP3 -> SHL -> IMAD -> IMAD.WIDE per byte instead of LOP3 -> IMAD.WIDE: a three times longer dependent chain)
   uint32_t lo2, carry;
   asm("{\n\t.reg .u64 t;\n\tmul.wide.u32 t, %2, 435;\n\tmov.b64 {%0, %1}, t;\n\t}" : "=r"(lo2), "=r"(carry) : "r"(x));
   h.hi = h.hi * 0x1b3u + (carry + (x << 8));
@@ -245,9 +245,8 @@ __global__ void __launch_bounds__(128) hash_chain_kernel(const uint32_t* __restr
 
 // Two-warp variant for block sizes <= 16 (the vLLM default is 16): 32 chains per CTA, warp 0 STAGES block i+1 of
 // every chain (pass 1) while warp 1 FOLDS block i (pass 2), double-buffered strips, one CTA barrier per block.
-// The two warps sit on different SM sub-partitions, so the encode work leaves the serial chain's issue stream:
-// measured on B200 the one-warp kernel is issue-bound (1048 instructions per block at 3.1 cycles per instruction
-// for a lone warp, profiles/r01_ncu_hash_*.txt).
+// The two warps sit on different SM sub-partitions, so the encode work leaves the serial chain's issue stream: the
+// one-warp kernel is issue-bound (a lone in-order warp retires about one instruction per three cycles).
 template <int BS, bool BRANCH_FREE>
 __global__ void __launch_bounds__(64) hash_chain_kernel_2w(const uint32_t* __restrict__ tokens,
                                                            const int64_t* __restrict__ prompt_off,
@@ -375,7 +374,10 @@ constexpr uint64_t kFnvPrimeInv = inv_mod_2_64(kFnvPrime);
 static_assert(kFnvPrimeInv * kFnvPrime == 1ull, "P^-1 mod 2^64");
 constexpr int kWpcPositions = 96;  // 32 lanes x 3 stream positions
 constexpr int kWpcPrefix = 11;     // 83 1b P7..P0 (80+BS)
-constexpr int kWpcMaxPrompts = 1536;  // beyond ~2000 prompts the lane-per-prompt kernels (flat ~66 us to 19k) win
+// The warp-per-prompt kernel takes batches of up to kWpcPromptsPerSm prompts per SM; past that the SMs are full and the
+// lane-per-prompt kernels win (H100, 132 SMs, tests/bench_hash.py: 58 vs 63 us at 1320 prompts, even at 1408, 65 vs
+// 62 us at 1536)
+constexpr int kWpcPromptsPerSm = 10;
 constexpr int kChainMaxPrompts = 1536; // round-2 chain kernel; the round-1 warp kernel stays available (KVB_HASH_KERNEL=wpc)
 
 __device__ __forceinline__ uint64_t pow_u64(uint64_t base, uint32_t e) {  // e < 128
@@ -662,7 +664,7 @@ __global__ void __launch_bounds__(64) hash_chain_kernel_wpc(const uint32_t* __re
 //     stager resolves them for the stream with the parent bytes ZEROED (six ballots, off the chain) and the folder adds
 //     the parent's contribution with two 64-bit masks per position and one popcount each: six vote rounds instead of
 //     eight, at the price of more instructions in both warps.
-// A lone in-order warp retires about one instruction per three cycles (profiles/r02_hash_phase_v2.txt), so the
+// A lone in-order warp retires about one instruction per three cycles (tools/micro/hash_phase_profile.cu), so the
 // folder's INSTRUCTION COUNT is on the chain as much as its dependency depth: everything that does not depend on the
 // parent key is done by the stagers.  The arithmetic is restated on the CPU in tests/test_wpc_math.py.
 constexpr int kV2Slots = 4;    // staged blocks the stagers may run ahead
@@ -701,7 +703,7 @@ template <int BS, bool MERGED, bool SCORE, int CHUNK_TOK = 128, int LOOKAHEAD = 
 __global__ void __launch_bounds__(32 * (2 + (SCORE ? 1 : 0))) chain_kernel(const ChainArgs A) {
   static_assert(BS > 0 && BS < 24 && kWpcPrefix + 5 * BS + 1 <= kWpcPositions, "stream must fit 96 positions");
   constexpr uint32_t kFull = 0xffffffffu;
-  constexpr int NST = 1;  // one stager warp keeps up (two were measured: no gain, profiles/r02_hash_time_c.json)
+  constexpr int NST = 1;  // one stager warp keeps up (a second one gains nothing: tests/bench_hash.py)
   constexpr int S = kV2Slots, NT = 32 * (1 + NST + (SCORE ? 1 : 0));
   // token chunks: CHUNK_TOK tokens each (CHUNK_TOK / 128 16-byte granules per lane), LOOKAHEAD chunks in flight beyond
   // the one being consumed, ring of the next power of two >= LOOKAHEAD + 2 chunks
@@ -762,8 +764,8 @@ __global__ void __launch_bounds__(32 * (2 + (SCORE ? 1 : 0))) chain_kernel(const
     // 4 B copies of the tokens that are inside it
     const uint32_t* tk = A.tokens + t0;
     // The chunk grid is aligned to 128 B lines, not just to the 16 B granule: sysmem is read a line at a time, and a chunk
-    // that straddles lines makes the link fetch its boundary lines twice (tools/micro/pinned_read_bw.cu: 1024 prompts of
-    // 4000 B in 512 B chunks — 105 us on a 16 B grid, 87 us on a 128 B grid, 86 us for a plain streaming read)
+    // that straddles lines makes the link fetch its boundary lines twice (tools/micro/pinned_read_bw.cu compares the
+    // grids with a plain streaming read)
     const int mis = (int)((reinterpret_cast<uintptr_t>(tk) >> 2) & 31u);  // tokens between the 128 B boundary and tk
     const uint32_t* tka = tk - mis;
     const int need_hi = mis + nblk * BS;                                  // aligned token indices [mis, need_hi) are needed
@@ -795,7 +797,7 @@ __global__ void __launch_bounds__(32 * (2 + (SCORE ? 1 : 0))) chain_kernel(const
       if (i >= S)
         while (ld_acquire_cta(&folded) < i - S + 1) __nanosleep(64);  // until the slot's previous block is consumed
       // (waiting warps sleep instead of spinning: at 1024 prompts five warps share a scheduler and a spinning one takes
-      //  issue slots from a folding one — profiles/r02_ncu_index_raw.csv: 45.7 M instructions, most of them polls)
+      //  issue slots from a folding one, and most of the kernel's instructions become polls)
       __syncwarp();  // a chunk is written by all lanes and read by others
       const uint32_t t = lane < BS ? tring[(mis + i * BS + lane) & (kRingTok - 1)] : 0u;
       const bool ge24 = t >= 24u, ge256 = t >= 0x100u, ge64k = t >= 0x10000u;
@@ -865,8 +867,7 @@ __global__ void __launch_bounds__(32 * (2 + (SCORE ? 1 : 0))) chain_kernel(const
       rec[buf][1][lane] = make_uint4(chi[1], clo[2], chi[2], (uint32_t)n_tot | (text ? 0x80000000u : 0u));
       // Publish with a plain store after the warp barrier — NOT st.release: a release compiles to MEMBAR.ALL.CTA, and the
       // membar waits for every memory operation this warp has in flight, i.e. for the token chunks being prefetched from
-      // host memory.  That serialised each block behind a PCIe round trip (ncu: 685 membar-stall samples, 37 GB/s over
-      // PCIe instead of the link's 51).  Ordering still holds: the record stores of all lanes precede the barrier, the
+      // host memory.  That serialised each block behind a PCIe round trip.  Ordering still holds: the record stores of all lanes precede the barrier, the
       // counter store follows it, and one SM's shared-memory pipeline performs them in that order; readers poll the
       // counter before they load the record.
       __syncwarp();
@@ -1071,8 +1072,9 @@ __global__ void __launch_bounds__(32 * (2 + (SCORE ? 1 : 0))) chain_kernel(const
 
 template <int BS, bool SCORE>
 static void launch_chain_bs(const ChainArgs& a, int n_prompts, cudaStream_t s) {
-  // MERGED (bits 0/1 without votes) shortens a lone chain by ~2 us but costs instructions in both warps: it pays while
-  // every folder has a scheduler to itself and loses when they share one (profiles/r02_hash_time_c.json).  A/B: KVB_HASH_MERGED
+  // MERGED (bits 0/1 without votes) shortens a lone chain but costs instructions in both warps: it pays while every
+  // folder has a scheduler to itself and loses when they share one.  On H100 the two measure the same from 16 to 2048
+  // prompts (tests/bench_hash.py), so the switch point is kept.  A/B: KVB_HASH_MERGED
   const char* e2 = std::getenv("KVB_HASH_MERGED");
   const bool merged = e2 ? std::atoi(e2) != 0 : n_prompts <= 512;
   // token fetch geometry (A/B: KVB_CHAIN_FETCH = 128x2 | 256x2 | 256x4 | 128x6): chunk size in tokens x chunks ahead
@@ -1114,7 +1116,7 @@ bool launch_chain_score(const ChainArgs& a, int32_t n_prompts, int32_t block_siz
 // the chain.  So fold(v, tail) is tabulated for all 256 values of v — 256 independent plain FNV runs per block, in
 // parallel over every block of every prompt (phase A: one 128-thread CTA per block, two start values per thread) —
 // and the serial chain per block shrinks to the 10 prefix bytes plus one table look-up and one multiply by P^m (phase B:
-// one thread per prompt): 309 cycles per block measured, against ~1000 for the vote rounds.  The price is 256x the byte
+// one thread per prompt): about a third of the cycles per block of the vote rounds.  The price is 256x the byte
 // work, which idle SMs absorb for small batches only (the vote kernels stay the choice from a few dozen prompts up).
 constexpr int kSpecThreads = 128;   // each thread folds TWO start values (two independent chains: the warp's issue slots
                                     // are half empty with one), so a 128-thread CTA tabulates a block
@@ -1123,7 +1125,8 @@ constexpr int kSpecPassRows = 8;    // table rows (blocks) per staging buffer; t
 constexpr int kSpecChunk = 640;     // tail bytes staged per round (128 tokens x 5 B)
 constexpr int kSpecMaxPrompts = 64;
 constexpr int kSpecAutoPrompts = 16;  // the small argument block holds this many prompts
-constexpr int kSpecDefaultPrompts = 32;  // chosen without being asked for up to this many prompts
+constexpr int kSpecDefaultPrompts = 32;  // chosen without being asked for up to this many prompts (H100 fused call,
+                                          // tests/bench_small_batches.py: 47 vs 53 us at 32 prompts, 62 vs 55 us at 64)
 constexpr int kSpecKeyRing = 64;
 
 struct SpecArgs {
@@ -1601,8 +1604,8 @@ bool launch_spec_score(const ChainArgs& a, int32_t n_prompts, int32_t block_size
                        SpecScratch* scratch) {
   *rc_out = KVB_OK;
   if (!spec_wanted(n_prompts)) return false;
-  // this chain hands over a key every ~0.16 us, a probe round costs ~1.5 us whatever its size: the scorer takes full
-  // tiles (with the vote-round chain, four times slower, small tiles keep it closer behind)
+  // this chain hands over keys far faster than a probe round completes, whatever the round's size: the scorer takes
+  // full tiles (with the slower vote-round chain, small tiles keep it closer behind)
   ChainArgs b = a;
   const char* e = std::getenv("KVB_SPEC_SCORE_BATCH");
   b.score_min_batch = e ? std::max(1, std::min(32, std::atoi(e))) : 32;
@@ -1640,15 +1643,17 @@ int launch_hash_blocks(const uint32_t* tokens, const int64_t* prompt_off, const 
     if (launch_spec(a, false, n_prompts, block_size, total_keys, s, &rc, h_prompt_off, h_key_off, h_parents, scratch)) return rc;
   }
   // small batches: 32-thread CTAs so the chains spread over the SMs; large: 128
-  const int threads = n_prompts >= 148 * 128 ? 128 : 32;
+  int dev = 0;
+  cudaGetDevice(&dev);
+  const int threads = n_prompts >= sm_count(dev) * 128 ? 128 : 32;
   const int grid = (n_prompts + threads - 1) / threads;
   static const bool one_warp = std::getenv("KVB_HASH_ONE_WARP") != nullptr;  // A/B switch for profiling
   // KVB_HASH_KERNEL=lanes forces the lane-per-prompt kernels (A/B and parity tests of both families); read per call
   const char* force = std::getenv("KVB_HASH_KERNEL");
   const bool lanes_only = force != nullptr && std::strcmp(force, "lanes") == 0;
   const bool wpc_v1 = force != nullptr && std::strcmp(force, "wpc") == 0;  // round-1 warp kernel, kept for A/B
-  // the round-2 chain kernel in its hash-only form: measured no faster than round 1's warp kernel (36.9 vs 34.8 us for one
-  // prompt, 51 vs 47 us for 1024), so it hashes alone only on request; its value is the fused tokens -> scores launch
+  // the round-2 chain kernel in its hash-only form is no faster than round 1's warp kernel (tests/bench_hash.py), so it
+  // hashes alone only on request; its value is the fused tokens -> scores launch
   const bool chain_only = force != nullptr && std::strcmp(force, "chain") == 0;
   if (chain_only && n_prompts <= kChainMaxPrompts && chain_kernel_supports(block_size)) {
     ChainArgs a{};
@@ -1672,7 +1677,7 @@ int launch_hash_blocks(const uint32_t* tokens, const int64_t* prompt_off, const 
     count_launch();
     return KVB_OK;
   }
-  if (!one_warp && !lanes_only && n_prompts <= kWpcMaxPrompts && (block_size == 16 || block_size == 8 || block_size == 4)) {
+  if (!one_warp && !lanes_only && n_prompts <= kWpcPromptsPerSm * sm_count(dev) && (block_size == 16 || block_size == 8 || block_size == 4)) {
     if (block_size == 16)
       hash_chain_kernel_wpc<16><<<n_prompts, 64, 0, s>>>(tokens, prompt_off, parents, extra, extra_off, out_keys, key_off);
     else if (block_size == 8)
@@ -1689,8 +1694,6 @@ int launch_hash_blocks(const uint32_t* tokens, const int64_t* prompt_off, const 
   }
   const int grid2 = (n_prompts + 31) / 32;
   // fewer CTAs than ~2 per SM sub-partition: every warp is alone on its scheduler -> optimise latency, else issue slots
-  int dev = 0;
-  cudaGetDevice(&dev);
   const bool latency_bound = grid2 <= 4 * sm_count(dev);
   switch (one_warp ? -1 : block_size) {
 #define KVB_LAUNCH_2W(BSV)                                                                                          \
@@ -1873,7 +1876,7 @@ int kvb_hash_token_blocks(int device, const uint32_t* tokens, const int64_t* pro
     std::memcpy(H + o_koff, out_key_off, ((size_t)n_prompts + 1) * 8);
     std::memcpy(H + o_par, parents, (size_t)n_prompts * 8);
     // tokens go straight from the caller's buffer: pinned memory is read by the copy engine in place, pageable memory
-    // is staged by the driver (measured faster than staging it here: 0.34 vs 0.38-0.43 ms for 4 MB, tools/ab_stage.py)
+    // is staged by the driver (faster than staging it here: tools/ab_stage.py compares the two)
     KVB_CUDA_TRY(cudaMemcpyAsync(D + o_tok, tokens + prompt_off[0], (size_t)total_tok * 4, cudaMemcpyHostToDevice, s));
     KVB_CUDA_TRY(cudaMemcpyAsync(D + o_poff, H + o_poff, small_end - o_poff, cudaMemcpyHostToDevice, s));
     if (extra_off) {

@@ -33,8 +33,8 @@ int sm_count(int device) {
   static bool have[64];
   std::lock_guard<std::mutex> lk(mu);
   if (device >= 0 && device < 64 && have[device]) return cache[device];
-  int n = 148;
-  if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, device) != cudaSuccess || n <= 0) n = 148;
+  int n = 132;
+  if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, device) != cudaSuccess || n <= 0) n = 132;
   if (device >= 0 && device < 64) {
     cache[device] = n;
     have[device] = true;

@@ -17,7 +17,7 @@ class StorageOffloadEngine:
     """Async KV-block offload between the GPU KV cache and a storage tier.
 
     Positional arguments are the reference's (storage_offload_bindings.cpp:30-41).  Keyword-only
-    extensions select the B200-native host tier:
+    extensions select the H100-native host tier:
       tier="file"        reference on-disk format under the given file paths (default, drop-in)
       tier="host_arena"  pinned host DRAM arena of ``host_arena_bytes`` keyed by the same path strings
     ``gds_mode`` (file tier) takes the reference's strings (gds_file_io.cpp:425-446): reads and/or writes then use its

@@ -4,7 +4,7 @@ Mirror of pkg/kvevents (pool.go:253-398 processEventBatch, :206-249 realignExtra
 (engineadapter/vllm_adapter.go:64-260, common.go:34-130).  Transport (ZMQ subscribe, pod discovery) stays out of
 scope: callers hand in (topic, payload) pairs or decoded events.
 
-B200-first addition: `EventProcessor.process_many` takes the pending batches of MANY pods and hashes one BlockStored
+GPU-first addition: `EventProcessor.process_many` takes the pending batches of MANY pods and hashes one BlockStored
 event per pod per round in a single device call (events of one pod stay in order, pods are independent — the
 reference runs them on parallel worker shards, pool.go:154-166)."""
 from __future__ import annotations

@@ -16,6 +16,6 @@ Parity status (see DESIGN.md "Oracle"):
                             (scores 3.0 / 2.5 / 1.8 ..., transcribed in tests/).
   * offload staging/file — no golden bytes exist in the reference (layout is only
                             pinned by read-after-write symmetry); the layout is
-                            restated from the code and cross-checked on the GPU box
-                            against the reference engine built in oracle/_ref.
+                            restated from the code and cross-checked against files
+                            the reference engine wrote (tests/golden/ref_offload_files.json).
 """

@@ -5,8 +5,8 @@ cites the reference file:line (relative to /root/reference/kv_connectors/llmd_fs
 
 The reference holds no golden *bytes* for this path (its tests only check that a load
 returns what a store wrote, tests/test_fs_backend.py:353-411), so this layout statement is
-taken from the code; on the GPU box tests/test_offload_ref_interop.py cross-checks it
-against files written by the reference engine itself (oracle/_ref).
+taken from the code; tests/test_gpu_ref_interop.py cross-checks it against files written by the reference
+engine itself (stored under tests/golden/).
 """
 from __future__ import annotations
 

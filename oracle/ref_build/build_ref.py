@@ -3,9 +3,9 @@
 
 Compiles the reference's own sources *where they lie* under /root/reference
 (kv_connectors/llmd_fs_backend/csrc/storage, source list = its setup.py:21-30) with
-torch.utils.cpp_extension for sm_100a.  Nothing is copied into this repo; the only
+torch.utils.cpp_extension for sm_90a.  Nothing is copied into this repo; the only
 addition is shim/numa.h (libnuma is absent from the image, see the header).
-Output: oracle/_ref/storage_offload_ref.so  (git-ignored, travels with gpurun).
+Output: oracle/_ref/storage_offload_ref.so  (git-ignored).
 
 Used by bench.py --impl reference and bench.py's cpu_baseline leg as the reference arm.
 """
@@ -45,7 +45,7 @@ def build(verbose: bool = False) -> str | None:
     for var, exe in (("CXX", "/usr/bin/g++"), ("CC", "/usr/bin/gcc")):
         if os.path.exists(exe):
             os.environ[var] = exe
-    os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "10.0a")
+    os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "9.0a")
     os.environ.setdefault("MAX_JOBS", "8")
     from torch.utils.cpp_extension import load
 

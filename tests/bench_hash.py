@@ -19,7 +19,7 @@ def main():
     torch.cuda.set_device(0)
     kvb = importlib.import_module("llm-d-kv-cache_b200")
     lib = kvb.lib
-    sizes = [int(x) for x in sys.argv[1:]] or [1, 4, 16, 64, 148, 1024]
+    sizes = [int(x) for x in sys.argv[1:]] or [1, 4, 16, 64, 132, 1024]
     bs, ntok = 16, 1000
     rng = np.random.default_rng(2)
     out = {}

@@ -144,14 +144,14 @@ def main():
     assert np.array_equal(d_keys.cpu().numpy().view(np.uint64), keys_c), "device-resident hash differs from the oracle"
     # latency floors (DESIGN.md section 4), all chains concurrent so the LONGEST chain bounds the launch:
     #  - byte-serial formulation (lane per prompt): one dependent xor -> 64-bit multiply per CBOR byte, 12.3 cycles per
-    #    byte on a lone in-order warp (profiles/r01_hash_phase_profile.txt)
+    #    byte on a lone in-order warp (model constant; tools/micro/hash_phase_profile.cu measures it)
     #  - vote-round formulation (warp per prompt, the kernel used for <= 1536 prompts): per block 8 rounds of
     #    IMAD -> LOP3 -> LOP3.P -> VOTE -> LOP3 -> POPC -> SHL -> LOP3 (61 cycles) + 4x REDUX and recombine (80) + the
-    #    64-bit multiply (15)  (profiles/r01_warp_chain_latency.txt)
+    #    64-bit multiply (15)  (model constants; tools/micro/warp_chain_latency.cu measures them)
     full = tokens.reshape(N_PROMPTS, N_TOK)[:, : (N_TOK // BS) * BS]
     width = np.where(full < 24, 1, np.where(full < 256, 2, np.where(full < 65536, 3, 5)))
     chain_bytes = width.sum(axis=1) + (N_TOK // BS) * (1 + 9 + 1 + 1)        # 0x83, uint64 parent, array head, null extra
-    sm_hz = 1.965e9
+    sm_hz = 1.98e9   # H100 SXM maximum SM clock
     byte_floor = float(chain_bytes.max()) * 12.3 / sm_hz
     vote_floor = (N_TOK // BS) * (8 * 61 + 80 + 15) / sm_hz
     cores = os.cpu_count() or 1

@@ -105,7 +105,7 @@ def test_long_context_chain_property(kvb, torch_cuda):
     assert sample == full[:100]
 
 
-@pytest.mark.parametrize("n_prompts", [1, 31, 1536, 1537, 5000])
+@pytest.mark.parametrize("n_prompts", [1, 31, 1320, 1321, 1536, 1537, 5000])
 def test_dispatch_boundary_batches_match_c_oracle(kvb, torch_cuda, n_prompts):
     """Batch sizes either side of the warp-per-chain / lane-per-prompt dispatch threshold, ragged lengths, mixed token
     widths and short parents, against the oracle's C restatement."""

@@ -60,7 +60,7 @@ def _worker(rank, world, port, q):
 def test_ring_migration_two_gpus(torch_cuda):
     torch = torch_cuda
     if torch.cuda.device_count() < 2:
-        pytest.skip("needs 2 GPUs (run under gpurun --gpus 2)")
+        pytest.skip("needs 2 GPUs")
     import torch.multiprocessing as mp
     world = 2
     ctx = mp.get_context("spawn")

@@ -1,7 +1,11 @@
-"""Interop with the UNMODIFIED reference engine (oracle/_ref, built from /root/reference's own csrc): files written
-by one implementation are loaded by the other, and both on-disk images equal the oracle's layout statement.
-This is what pins oracle/offload_oracle.py (the reference holds no golden bytes for this path)."""
-import importlib.util
+"""Interop with the unmodified reference engine, pinned by the bytes it wrote.  tests/golden/ref_offload_files.json
+holds, per file the reference engine (kv_connectors/llmd_fs_backend, built by oracle/ref_build) stored for the inputs
+below, its size, the payload's offset and the SHA-256 of the payload; tests/golden/make_ref_offload_golden.py recorded
+them.  Our files must carry the same bytes, and files laid out as the reference writes them must load back through our
+engine.  This is what pins oracle/offload_oracle.py (the
+reference's own tests hold no golden bytes for this path)."""
+import hashlib
+import json
 import os
 import shutil
 import time
@@ -12,19 +16,18 @@ import pytest
 from oracle import offload_oracle as oo
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-SO = os.path.join(ROOT, "oracle", "_ref", "storage_offload_ref.so")
+GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 TMP = "/tmp/kvb-ref-interop"
 
 
-@pytest.fixture(scope="module")
-def ref_mod(torch_cuda):
-    if not os.path.exists(SO):
-        pytest.skip("oracle/_ref not built (needs /root/reference at build time)")
-    spec = importlib.util.spec_from_file_location("storage_offload_ref", SO)
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
+def cpu_case(bpf):
+    """Inputs of the CPU-path case: T tensors of (N, frag) bytes and three files, the first one partial."""
+    T, N, frag = 6, 48, 8192
+    rng = np.random.default_rng(11)
+    src = [rng.integers(0, 256, (N, frag), dtype=np.uint8) for _ in range(T)]
+    ids = [[5, 9][:bpf] if bpf > 1 else [5], list(range(10, 10 + bpf)), list(range(30, 30 + bpf))]
+    ids[0] = ids[0][: max(1, bpf // 2)]
+    return src, ids
 
 
 def _drain(eng, job):
@@ -37,90 +40,51 @@ def _drain(eng, job):
     raise TimeoutError(job)
 
 
-@pytest.mark.parametrize("bpf", [1, 4])
-def test_files_interoperate_and_match_oracle(kvb, torch_cuda, ref_mod, bpf):
-    torch = torch_cuda
-    shutil.rmtree(TMP, ignore_errors=True)
-    T, N, frag = 6, 48, 8192
-    g = torch.Generator(device="cuda").manual_seed(11)
-    src = [torch.randint(-128, 127, (N, frag), dtype=torch.int8, device="cuda", generator=g) for _ in range(T)]
-    np_src = [t.cpu().numpy().view(np.uint8) for t in src]
-    ids = [[5, 9][:bpf] if bpf > 1 else [5], list(range(10, 10 + bpf)), list(range(30, 30 + bpf))]
-    ids[0] = ids[0][: max(1, bpf // 2)]                       # partial first file
-    ref = ref_mod.StorageOffloadEngine(4, bpf, src, 3, "disabled", 0.0)
-    ours = kvb.engine.StorageOffloadEngine(4, bpf, src, 3, "disabled", 0.0)
-    f_ref = [f"{TMP}/ref/{i}.bin" for i in range(3)]
-    f_our = [f"{TMP}/ours/{i}.bin" for i in range(3)]
-    ref.async_store_gpu_blocks(1, f_ref, ids)
-    assert _drain(ref, 1)
-    assert ours.async_store_gpu_blocks(1, f_our, ids)
-    assert _drain(ours, 1)
-    for fr, fo, blk in zip(f_ref, f_our, ids):
-        a, b = np.fromfile(fr, dtype=np.uint8), np.fromfile(fo, dtype=np.uint8)
-        want = oo.file_image(np_src, blk, bpf)
-        assert a.size == b.size == want.size == oo.staging_size(T, frag, bpf)
-        off = oo.slot_offset(T, frag, bpf, len(blk))
-        n = len(blk) * T * frag
-        # payload region identical in all three; outside it the reference holds stale staging bytes, we hold zeros
-        assert np.array_equal(a[off:off + n], want[off:off + n]) and np.array_equal(b, want)
-    # cross loads into zeroed caches
-    for writer_files, reader_name in ((f_ref, "ours"), (f_our, "ref")):
-        dst = [torch.zeros_like(t) for t in src]
-        eng = (kvb.engine.StorageOffloadEngine(2, bpf, dst, 1, "disabled", 0.0) if reader_name == "ours"
-               else ref_mod.StorageOffloadEngine(2, bpf, dst, 1, "disabled", 0.0))
-        eng.async_load_gpu_blocks(2, writer_files, ids)
-        assert _drain(eng, 2)
-        torch.cuda.synchronize()
+def _device(torch, np_src):
+    return [torch.from_numpy(a).view(torch.int8).cuda() for a in np_src]
+
+
+def _loads_back(kvb, torch, src, bpf, files, ids):
+    dst = [torch.zeros_like(t) for t in src]
+    eng = kvb.engine.StorageOffloadEngine(2, bpf, dst, 1, "disabled", 0.0)
+    assert eng.async_load_gpu_blocks(2, files, ids)
+    assert _drain(eng, 2)
+    torch.cuda.synchronize()
+    for blk in ids:
         for d, s in zip(dst, src):
-            for blk in ids:
-                for b in blk:
-                    assert torch.equal(d[b], s[b]), (reader_name, b)
-        if reader_name == "ours":
-            eng.shutdown()
-        del eng
-    ours.shutdown()
-    del ref
-    shutil.rmtree(TMP, ignore_errors=True)
+            assert torch.equal(d[blk], s[blk])
+    eng.shutdown()
 
 
-def test_gds_files_interoperate(kvb, torch_cuda, ref_mod):
-    """gds_mode="read_write" on both sides: the reference writes its GDS format through cuFile (compatibility mode when
-    nvidia-fs is absent), we load it — and the other way round; the file bytes are identical."""
+@pytest.mark.parametrize("bpf", [1, 4])
+def test_files_interoperate_and_match_oracle(kvb, torch_cuda, bpf):
     torch = torch_cuda
-    root = "/dev/shm/kvb-ref-interop-gds"
-    shutil.rmtree(root, ignore_errors=True)
-    T, N, frag, bpf = 4, 32, 8192, 4
-    g = torch.Generator(device="cuda").manual_seed(12)
-    src = [torch.randint(-128, 127, (N, frag), dtype=torch.int8, device="cuda", generator=g) for _ in range(T)]
-    np_src = [t.cpu().numpy().view(np.uint8) for t in src]
-    ids = [[5, 9], [10, 11, 12, 13], [31, 30, 29, 28]]
-    ref = ref_mod.StorageOffloadEngine(4, bpf, src, 3, "read_write", 0.0)
-    ours = kvb.engine.StorageOffloadEngine(4, bpf, src, 3, "read_write", 0.0)
-    f_ref = [f"{root}/ref/{i}.bin" for i in range(3)]
-    f_our = [f"{root}/ours/{i}.bin" for i in range(3)]
-    ref.async_store_gpu_blocks(1, f_ref, ids)
-    ref_ok = _drain(ref, 1)
+    shutil.rmtree(TMP, ignore_errors=True)
+    np_src, ids = cpu_case(bpf)
+    T, frag = len(np_src), np_src[0].shape[1]
+    src = _device(torch, np_src)
+    with open(os.path.join(GOLDEN, "ref_offload_files.json")) as fh:
+        gold = json.load(fh)[f"bpf{bpf}"]
+    ours = kvb.engine.StorageOffloadEngine(4, bpf, src, 3, "disabled", 0.0)
+    f_our = [f"{TMP}/ours/{i}.bin" for i in range(3)]
     assert ours.async_store_gpu_blocks(1, f_our, ids)
     assert _drain(ours, 1)
-    # the reference has no I/O-time fallback: when cuFileHandleRegister fails (error 5030 on the GPU boxes' overlay and
-    # tmpfs mounts) its write task logs the error and leaves no file behind; our files are still checked below
-    for fo, blk in zip(f_our, ids):
-        assert np.array_equal(np.fromfile(fo, dtype=np.uint8), oo.pack_blocks(np_src, blk))
-    if not ref_ok or not all(os.path.exists(f) for f in f_ref) or os.path.getsize(f_ref[0]) != len(ids[0]) * T * frag:
-        pytest.skip("the reference engine's GDS path is not usable on this box / file system")
-    for fr, fo, blk in zip(f_ref, f_our, ids):
-        a, b = np.fromfile(fr, dtype=np.uint8), np.fromfile(fo, dtype=np.uint8)
-        assert np.array_equal(a, b) and np.array_equal(b, oo.pack_blocks(np_src, blk))
-    for writer_files, reader_name in ((f_ref, "ours"), (f_our, "ref")):
-        dst = [torch.zeros_like(t) for t in src]
-        eng = (kvb.engine.StorageOffloadEngine(2, bpf, dst, 1, "read_write", 0.0, strict_load_errors=True)
-               if reader_name == "ours" else ref_mod.StorageOffloadEngine(2, bpf, dst, 1, "read_write", 0.0))
-        eng.async_load_gpu_blocks(2, writer_files, ids)
-        assert _drain(eng, 2)
-        torch.cuda.synchronize()
-        for blk in ids:
-            for d, s in zip(dst, src):
-                assert torch.equal(d[blk], s[blk]), reader_name
-        del eng
-    del ref, ours
-    shutil.rmtree(root, ignore_errors=True)
+    ours.shutdown()
+    os.makedirs(f"{TMP}/ref")
+    f_ref = [f"{TMP}/ref/{i}.bin" for i in range(3)]
+    assert len(gold) == len(ids)
+    for ref, fo, fr, blk in zip(gold, f_our, f_ref, ids):
+        b = np.fromfile(fo, dtype=np.uint8)
+        want = oo.file_image(np_src, blk, bpf)
+        off, n = oo.slot_offset(T, frag, bpf, len(blk)), len(blk) * T * frag
+        assert ref["size"] == b.size == want.size == oo.staging_size(T, frag, bpf)
+        assert ref["offset"] == off and ref["payload_bytes"] == n
+        # payload region identical in all three; outside it the reference holds stale staging bytes, we hold zeros
+        assert hashlib.sha256(b[off:off + n].tobytes()).hexdigest() == ref["payload_sha256"] and np.array_equal(b, want)
+        img = np.full(b.size, 0xA5, dtype=np.uint8)       # the reference's file: its payload amid stale bytes
+        img[off:off + n] = b[off:off + n]
+        img.tofile(fr)
+    # files as either implementation wrote them load back into zeroed caches
+    for files in (f_ref, f_our):
+        _loads_back(kvb, torch, src, bpf, files, ids)
+    shutil.rmtree(TMP, ignore_errors=True)

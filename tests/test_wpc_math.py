@@ -80,7 +80,7 @@ def test_block_streams_of_the_kernel_shape():
 
 
 def test_three_redux_limb_split_is_exact():
-    """Variant tried in round 1 (DESIGN.md section 9.1: correct, not faster): sum the 32 lanes' 64-bit terms with THREE redux.sync.add.u32 instead of
+    """Variant tried in round 1 (correct, not faster): sum the 32 lanes' 64-bit terms with THREE redux.sync.add.u32 instead of
     four — 27-bit low limbs of both halves, and the two 5-bit tops packed into one word (10-bit fields: 32 * 31 < 1024)."""
     rng = random.Random(5)
     m27 = (1 << 27) - 1
@@ -97,7 +97,7 @@ def test_three_redux_limb_split_is_exact():
 
 
 def test_round_without_the_shift():
-    """Variant tried in round 1 (DESIGN.md section 9.1: correct, not faster): keep C_j = (resolved low bits of z_j) * 0xb3 as an accumulator and add
+    """Variant tried in round 1 (correct, not faster): keep C_j = (resolved low bits of z_j) * 0xb3 as an accumulator and add
     zeta * (0xb3 << k) per round, zeta = the newly resolved bit taken from the popcount's bit 0 — the parity then needs no
     shift on the vote -> popc -> vote chain.  Must resolve the same z bytes as the shipped formulation."""
     rng = random.Random(6)

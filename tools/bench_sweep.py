@@ -1,12 +1,12 @@
 #!/usr/bin/env python
 """BASELINE config #3: Llama-3-70B GQA paged-KV fp8-e4m3 (160 tensors x 16384 B, 2.5 MiB blocks), offload sweep.
 
-Resident pool N = 49152 blocks (128.8 GB of the 180 GB HBM).  For n in {1k, 4k, 16k, 48k}: device-resident
+Resident pool N = 16384 blocks (43 GB of the H100's 80 GB, beside a 21 GB packed slice).  For n in {1k, 4k, 16k}: device-resident
 gather/scatter timing (CUDA events per launch) and end-to-end save+load through the engine API (host-arena tier).
 {128k, 1M} blocks are CUMULATIVE: batches of 16k blocks cycled through a bounded 42 GB pinned arena
 (1 M x 2.5 MiB = 2.6 TB cannot be resident on the host tier at once) — stated, not hidden.
 One process per GPU under torchrun for the multi-GPU sweep (independent partitions, aggregate GB/s).
-Prints one JSON object on rank 0; kept under profiles/."""
+Prints one JSON object on rank 0."""
 import importlib
 import json
 import os
@@ -21,8 +21,8 @@ import torch  # noqa: E402
 
 T, FRAG = 160, 16384
 BLOCK = T * FRAG
-POOL = int(os.environ.get("KVB_SWEEP_POOL", "49152"))
-RESIDENT = [int(x) for x in os.environ.get("KVB_SWEEP_RESIDENT", "1000,4000,16000,48000").split(",")]
+POOL = int(os.environ.get("KVB_SWEEP_POOL", "16384"))
+RESIDENT = [int(x) for x in os.environ.get("KVB_SWEEP_RESIDENT", "1000,4000,16000").split(",")]
 CUMULATIVE = [int(x) for x in os.environ.get("KVB_SWEEP_CUMULATIVE", "128000,1000000").split(",") if x]
 BATCH = 16000
 BPF = 16

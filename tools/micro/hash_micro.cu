@@ -1,5 +1,5 @@
 // Micro-benchmark of the hash kernel's building blocks on one lone warp (cycles from clock64).
-// nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/micro/hash_micro tools/micro/hash_micro.cu
+// nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/micro/hash_micro tools/micro/hash_micro.cu
 #include <cstdint>
 #include <cstdio>
 #include <cuda_runtime.h>

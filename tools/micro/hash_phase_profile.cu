@@ -1,6 +1,6 @@
 // Per-phase cycle counts of the two-warp hash kernel (clock64 around each phase, CTA 0, lane 0).
 // (without -DKVB_HASH_PROFILE the same program only times the production kernel: tools/micro/hash_time)
-// nvcc -DKVB_HASH_PROFILE -gencode arch=compute_100a,code=sm_100a -O3 -I include -I llm-d-kv-cache_b200/csrc \
+// nvcc -DKVB_HASH_PROFILE -gencode arch=compute_90a,code=sm_90a -O3 -I include -I llm-d-kv-cache_b200/csrc \
 //      -o tools/micro/hash_phase_profile tools/micro/hash_phase_profile.cu llm-d-kv-cache_b200/csrc/pool_api.cu llm-d-kv-cache_b200/csrc/copy_kernels.cu
 #include "../../llm-d-kv-cache_b200/csrc/hash_kernels.cu"
 #include <vector>

@@ -2,7 +2,7 @@
 //   ldg  : 16 B per lane, a warp covers 512 B per instruction, ITEMS chunks per CTA
 //   cpas : cp.async.cg 16 B per lane into shared memory (what chain_kernel's stager does)
 //   bulk : cp.async.bulk (TMA, 1-D) of CHUNK bytes per elected thread into shared memory, mbarrier completion
-// against cudaMemcpyAsync (copy engine).   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/micro/pinned_read_bw tools/micro/pinned_read_bw.cu
+// against cudaMemcpyAsync (copy engine).   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/micro/pinned_read_bw tools/micro/pinned_read_bw.cu
 #include <cstdio>
 #include <cstdint>
 #include <cstdlib>
@@ -120,19 +120,21 @@ int main() {
     printf("%-44s %7.1f us  %6.1f GB/s\n", name, best * 1e3, bytes / (best * 1e-3) / 1e9);
   };
   time("cudaMemcpyAsync H2D (copy engine)", [&] { CK(cudaMemcpyAsync(d, h, bytes, cudaMemcpyHostToDevice, 0)); });
-  for (int grid : {148, 296, 1024}) for (int thr : {128, 256}) {
+  int sms = 0;
+  CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0));
+  for (int grid : {sms, 2 * sms, 1024}) for (int thr : {128, 256}) {
     char nm[96]; snprintf(nm, sizeof nm, "ldg 16 B/lane, grid %d x %d", grid, thr);
     time(nm, [&] { k_ldg<<<grid, thr>>>((const uint4*)h, bytes / 16, sink); });
   }
-  for (int grid : {148, 1024}) {
+  for (int grid : {sms, 1024}) {
     char nm[96]; snprintf(nm, sizeof nm, "cp.async 16 B/lane depth 8, grid %d x 128", grid);
     time(nm, [&] { k_cpas<8><<<grid, 128, 8 * 128 * 16>>>((const uint4*)h, bytes / 16, sink); });
   }
-  for (int grid : {148, 296, 592}) {
+  for (int grid : {sms, 2 * sms, 4 * sms}) {
     char nm[96]; snprintf(nm, sizeof nm, "cp.async.bulk 4000 B x 4 stages, grid %d", grid);
     time(nm, [&] { k_bulk<4000, 4><<<grid, 32, 4 * 4000>>>(h, bytes, sink); });
   }
-  for (int grid : {148, 296}) {
+  for (int grid : {sms, 2 * sms}) {
     char nm[96]; snprintf(nm, sizeof nm, "cp.async.bulk 16000 B x 4 stages, grid %d", grid);
     CK(cudaFuncSetAttribute(k_bulk<16000, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 4 * 16000));
     time(nm, [&] { k_bulk<16000, 4><<<grid, 32, 4 * 16000>>>(h, bytes, sink); });

@@ -1,7 +1,7 @@
 // Where do the warps of 1024 two-warp CTAs land?  Records (%smid, %warpid) of both warps of every CTA while all CTAs
 // are co-resident, then prints CTAs per SM and, per scheduler (warpid % 4), how many "folder" warps the hash kernel's
 // role rule would place there.
-// nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/micro/slot_map tools/micro/slot_map.cu
+// nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/micro/slot_map tools/micro/slot_map.cu
 #include <cstdio>
 #include <cstdint>
 #include <vector>

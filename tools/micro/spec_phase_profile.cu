@@ -1,6 +1,6 @@
 // Phase clocks of the table ("spec") hash kernel, CTA 0 (clock64 on one SM): start | own tables done | all tables seen |
 // first rows staged | chain start | chain end.
-// nvcc -DKVB_HASH_PROFILE -gencode arch=compute_100a,code=sm_100a -O3 -I include -I llm-d-kv-cache_b200/csrc \
+// nvcc -DKVB_HASH_PROFILE -gencode arch=compute_90a,code=sm_90a -O3 -I include -I llm-d-kv-cache_b200/csrc \
 //      -o tools/micro/spec_phase_profile tools/micro/spec_phase_profile.cu llm-d-kv-cache_b200/csrc/pool_api.cu llm-d-kv-cache_b200/csrc/copy_kernels.cu
 #include "../../llm-d-kv-cache_b200/csrc/hash_kernels.cu"
 #include <vector>

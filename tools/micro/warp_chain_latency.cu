@@ -1,6 +1,6 @@
 // Dependent-chain latencies of the warp-level instructions the warp-per-chain hash kernel is built from
 // (one warp, one CTA; clock64 around N dependent iterations).
-// nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/micro/warp_chain_latency tools/micro/warp_chain_latency.cu
+// nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/micro/warp_chain_latency tools/micro/warp_chain_latency.cu
 #include <cstdio>
 #include <cstdint>
 constexpr int N = 4096;

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Is GPUDirect Storage usable on this box?  Reports the nvidia-fs kernel module, what cuFileDriverOpen returns, and
 whether cuFileHandleRegister / cuFileWrite / cuFileRead work from device memory on a few file systems
-(round 1: module absent, driver opens in compatibility mode -> DESIGN.md section 9 item 3)."""
+(without the module the driver opens in compatibility mode, see csrc/engine.cu)."""
 import ctypes
 import os
 import subprocess

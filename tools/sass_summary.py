@@ -2,7 +2,7 @@
 """SASS evidence for the kernels of libkvb.so: per kernel, the counts of the mnemonics that prove what it is (bulk-copy /
 mbarrier for the TMA mover, 128-bit non-allocating loads for the LDG mover, vote / popc / redux for the hash chain,
 match / atomics for the index), followed by the full listing of the default gather kernel.
-    python tools/sass_summary.py > profiles/r02_sass_kernels.txt"""
+    python tools/sass_summary.py > sass_kernels.txt"""
 import collections
 import os
 import re
@@ -28,7 +28,7 @@ def main():
         if cur and re.search(r"/\*[0-9a-f]{4}\*/", line):
             kernels[cur].append(line)
     demangle = lambda n: subprocess.run(["c++filt", n], capture_output=True, text=True).stdout.strip() or n
-    print("SASS mnemonic counts per kernel of llm-d-kv-cache_b200/libkvb.so (sm_100a), cuobjdump -sass\n")
+    print("SASS mnemonic counts per kernel of llm-d-kv-cache_b200/libkvb.so (sm_90a), cuobjdump -sass\n")
     for name, lines in kernels.items():
         counts = collections.Counter()
         for ln in lines:
