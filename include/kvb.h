@@ -224,6 +224,10 @@ typedef struct kvb_pod_entry { /* kvblock.PodEntry, index.go:176-183 */
 } kvb_pod_entry_t;
 
 #define KVB_INDEX_MAX_PODS_PER_KEY 13 /* entries that fit one 64 B bucket */
+/* Pod ids are 0..65534: at most 65 535 distinct pods per index.  65535 is reserved: kvb_index_add and the BlockStored
+ * events of kvb_index_ingest_events refuse it (KVB_ERR_INVALID), so no entry ever carries it.  A caller whose pod filter
+ * names no known pod passes it as the filter: nothing matches, and found keys are still refreshed. */
+#define KVB_POD_NONE 0xffff
 #define KVB_KEY_ENGINE 0              /* index.go:155-161 */
 #define KVB_KEY_REQUEST 1
 

@@ -243,13 +243,8 @@ class Index {
                                                     const std::set<std::string>& podIdentifierSet = {}) {
     if (requestKeys.empty()) throw Error(KVB_ERR_INVALID, "no requestKeys provided for lookup");
     std::lock_guard<std::mutex> lk(mu_);
-    std::vector<uint16_t> filter;
-    for (const auto& name : podIdentifierSet) {
-      auto it = pods_.find(name);
-      if (it != pods_.end()) filter.push_back(it->second);
-    }
+    const std::vector<uint16_t> filter = podFilter(podIdentifierSet);
     std::map<BlockHash, std::vector<PodEntry>> out;
-    if (!podIdentifierSet.empty() && filter.empty()) return out;  // the filter names nobody the index has seen
     const size_t n = requestKeys.size();
     std::vector<int32_t> counts(n);
     std::vector<kvb_pod_entry_t> ents(n * KVB_INDEX_MAX_PODS_PER_KEY);
@@ -284,13 +279,8 @@ class Index {
     for (int32_t i = 0; i < n; ++i) std::copy(prompts[i].begin(), prompts[i].end(), flat.begin() + off[i]);
     std::vector<uint64_t> parents(n, init);
     std::lock_guard<std::mutex> lk(mu_);
-    std::vector<uint16_t> filter;
-    for (const auto& name : podIdentifiers) {
-      auto it = pods_.find(name);
-      if (it != pods_.end()) filter.push_back(it->second);
-    }
+    const std::vector<uint16_t> filter = podFilter(podIdentifiers);
     std::vector<std::map<std::string, double>> res(n);
-    if (!podIdentifiers.empty() && filter.empty()) return res;
     std::vector<int32_t> out_n(n);
     std::vector<uint16_t> out_p((size_t)n * KVB_INDEX_MAX_PODS_PER_KEY);
     std::vector<double> out_s((size_t)n * KVB_INDEX_MAX_PODS_PER_KEY);
@@ -304,12 +294,24 @@ class Index {
   }
 
  private:
+  // interned ids of the known names; a filter that names only unknown pods becomes {KVB_POD_NONE}: the kernels run,
+  // match nothing and still refresh every key they find, as the reference's Lookup does (in_memory.go:119-120)
+  template <typename Names>
+  std::vector<uint16_t> podFilter(const Names& names) const {
+    std::vector<uint16_t> filter;
+    for (const auto& name : names) {
+      auto it = pods_.find(name);
+      if (it != pods_.end()) filter.push_back(it->second);
+    }
+    if (!names.empty() && filter.empty()) filter.push_back(KVB_POD_NONE);
+    return filter;
+  }
   std::vector<kvb_pod_entry_t> intern(const std::vector<PodEntry>& in) {
     std::vector<kvb_pod_entry_t> out(in.size());
     for (size_t i = 0; i < in.size(); ++i) {
       auto p = pods_.find(in[i].PodIdentifier);
       if (p == pods_.end()) {
-        if (pod_names_.size() >= 65536) throw Error(KVB_ERR_UNSUPPORTED, "too many distinct pod identifiers");
+        if (pod_names_.size() >= KVB_POD_NONE) throw Error(KVB_ERR_UNSUPPORTED, "too many distinct pod identifiers");
         p = pods_.emplace(in[i].PodIdentifier, (uint16_t)pod_names_.size()).first;
         pod_names_.push_back(in[i].PodIdentifier);
       }

@@ -13,6 +13,7 @@ ABI_VERSION = 5
 COPY_DEFAULT, COPY_LDG, COPY_BULK = 0, 1, 2
 TIER_FILE, TIER_HOST_ARENA = 0, 1
 MAX_PODS_PER_KEY = 13
+NO_SUCH_POD = 0xFFFF  # KVB_POD_NONE: never an interned pod id
 KEY_ENGINE, KEY_REQUEST = 0, 1
 SCORE_TOUCH_LRU, SCORE_NO_TOUCH, SCORE_TIME_KERNELS, SCORE_COPY_TOKENS, SCORE_TWO_KERNELS, SCORE_PINNED_IO = 1, 2, 4, 8, 16, 32
 

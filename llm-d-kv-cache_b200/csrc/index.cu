@@ -1429,6 +1429,8 @@ int kvb_index_add(kvb_index_t* idx, const uint64_t* engine_keys, int64_t n_engin
                 "no keys or entries provided for adding to index");
     KVB_REQUIRE(!has_engine_keys || n_engine > 0, "engineKeys is non-nil but empty");
     KVB_REQUIRE(n_entries <= 65535, "too many entries in one Add");
+    for (int32_t i = 0; i < n_entries; ++i)  // the "no such pod" filter must never match a stored entry
+      KVB_REQUIRE(entries[i].pod != KVB_POD_NONE, "pod id %d is reserved (KVB_POD_NONE)", KVB_POD_NONE);
     std::lock_guard<std::mutex> lk(idx->mu);
     DeviceGuard g(idx->device);
     if (has_engine_keys) map_engine_keys(*idx->eng, engine_keys, n_engine, request_keys, n_request);  // in_memory.go:166-177
@@ -1497,6 +1499,8 @@ int kvb_index_ingest_events(kvb_index_t* idx, const kvb_kv_event_t* ev, int32_t 
     std::vector<std::vector<int32_t>> rounds;
     for (int32_t e = 0; e < n_events; ++e) {
       KVB_REQUIRE(ev[e].n_tokens >= 0 && ev[e].n_engine_keys >= 0, "event %d has negative sizes", e);
+      KVB_REQUIRE(ev[e].type != KVB_EVENT_BLOCK_STORED || ev[e].entry.pod != KVB_POD_NONE,
+                  "event %d: pod id %d is reserved (KVB_POD_NONE)", e, KVB_POD_NONE);
       const int32_t r = seen[ev[e].stream]++;
       if ((size_t)r >= rounds.size()) rounds.resize((size_t)r + 1);
       rounds[(size_t)r].push_back(e);

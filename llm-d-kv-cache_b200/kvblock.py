@@ -22,6 +22,7 @@ EMPTY_BLOCK_HASH = 0
 ENGINE_KEY = _lib.KEY_ENGINE
 REQUEST_KEY = _lib.KEY_REQUEST
 DEFAULT_BLOCK_SIZE = 16  # token_processor.go:32
+NO_SUCH_POD = _lib.NO_SUCH_POD  # reserved pod id: never assigned, the filter of a call that names no known pod
 
 
 # ------------------------------------------------------------------------------------------ extra keys
@@ -232,7 +233,7 @@ class Index:
         self._check(self._lib.kvb_index_create(self.device, int(size), int(pod_cache_size), int(expected_keys),
                                                C.byref(h)))
         self._h = h
-        self.pods = _Interner(65536, "pod identifiers")
+        self.pods = _Interner(NO_SUCH_POD, "pod identifiers")  # ids 0..65534
         self.tiers = _Interner(256, "device tiers")
         self._tier_lock = threading.Lock()
         self._weights: dict = {}
@@ -294,8 +295,8 @@ class Index:
         if not names:
             return None, 0
         ids = [self.pods.ids[n] for n in names if n in self.pods.ids]
-        if not ids:  # filter present but nothing known: use a never-assigned id so nothing matches
-            ids = [self.pods.get("\0__kvb_no_such_pod__")]
+        if not ids:  # filter present but nothing known: the reserved id matches nothing, found keys are still refreshed
+            ids = [NO_SUCH_POD]
         return np.asarray(ids, dtype=np.uint16), len(ids)
 
     def _entry_from_c(self, c) -> PodEntry:

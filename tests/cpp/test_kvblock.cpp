@@ -144,6 +144,23 @@ int main(int argc, char** argv) {
     auto batch = idx->ScoreTokensBatch(*tp, {toks, {1, 2}, {9, 9}}, model);
     CHECK(batch[0] == s && batch[1]["pod-a"] == 1.8 && batch[2].empty());
   }
+
+  // ---- a filter naming only unknown pods matches nothing but still refreshes what it finds (in_memory.go:119-120)
+  {
+    auto tp = std::make_shared<kvblock::TokenProcessor>(kvblock::TokenProcessorConfig{1, ""});
+    auto idx = std::make_shared<kvblock::Index>(kvblock::IndexConfig{3, 2});
+    kvcache::Indexer ix(tp, idx);
+    const std::string model = "test-model";
+    std::vector<uint64_t> k;
+    for (uint32_t t = 1; t <= 4; ++t) k.push_back(ix.ComputeBlockKeysFromTokens({t}, model).at(0));
+    for (int i = 0; i < 3; ++i) idx->Add(nullptr, {k[i]}, {{"pod-a", "gpu"}});  // full: k[0] is the oldest
+    auto none = ix.ScoreTokens({1}, model, {"nobody"});                         // finds k[0]: now the newest
+    CHECK(none.has_value() && none->empty());
+    CHECK(idx->Lookup({k[1]}, {"nobody", "nobody-else"}).empty());              // finds k[1]: newer than k[0]
+    idx->Add(nullptr, {k[3]}, {{"pod-a", "gpu"}});                             // evicts the oldest: k[2]
+    auto left = idx->Lookup({k[0], k[1], k[2], k[3]});
+    CHECK(left.size() == 3 && left.count(k[0]) && left.count(k[1]) && !left.count(k[2]) && left.count(k[3]));
+  }
   std::printf("OK %d checks\n", g_checks);
   return 0;
 }

@@ -129,6 +129,33 @@ def test_sequential_replay_stops_and_resumes_instead_of_scanning(sim):
     assert r.returncode == 0 and "resumes" in r.stdout, (r.stdout[-500:], r.stderr[-1500:])
 
 
+def test_unknown_only_filter_with_every_pod_id_taken(sim):
+    """Pod ids 0..65534 are assignable, 65535 is reserved and refused by kvb_index_add.  With all of them taken, a lookup
+    whose filter names only unknown pods returns {} (the reference returns an empty map) and still refreshes the keys
+    it finds."""
+    kvb, lib = sim
+    K = kvb.kvblock
+    idx = K.Index(size=3, pod_cache_size=2, expected_keys=16, lib=lib)
+    for i in range(65535):
+        assert idx.pods.get("p%d" % i) == i
+    with pytest.raises(OverflowError):
+        idx.pods.get("one-too-many")
+    e = [K.PodEntry("p65534", "gpu")]
+    for k in (1, 2, 3):
+        idx.add(None, [k], e)
+    assert idx.lookup([1, 99], ["nobody"]) == {}          # 1 is now the newest
+    assert len(idx.pods.names) == 65535
+    idx.add(None, [4], e)                                 # evicts 2
+    assert idx.lookup([1], ["p65534", "nobody"]) == {1: e}
+    assert set(idx.lookup([1, 2, 3, 4])) == {1, 3, 4}
+    reserved = (kvb._lib.PodEntryC * 1)()
+    reserved[0].pod = kvb._lib.NO_SUCH_POD                # no entry may carry the reserved id
+    k = np.asarray([5], dtype=np.uint64)
+    assert lib.kvb_index_add(idx._h, None, 0, 0, k.ctypes.data, 1, reserved, 1) == -1
+    assert set(idx.lookup([1, 2, 3, 4, 5])) == {1, 3, 4}
+    idx.close()
+
+
 def test_parallel_path_big_batches_growth_and_tombstones(sim):
     """No capacity pressure, batches of up to 400 keys with many repeats: sorted per-key replay, device-side rehash
     (the table starts at 2048 slots) and tombstone reuse."""
