@@ -89,7 +89,9 @@ int64_t kvb_pool_block_bytes(const kvb_pool_t* pool); /* T * frag_bytes */
  * defaults to the mover tuned for NVLink stores.  Auto-detected when the driver reports the owning device. */
 int kvb_pool_mark_peer(kvb_pool_t* pool, int is_peer);
 
-/* block_ids: HOST array of n ids.  packed: DEVICE (or device-mapped / peer) buffer of n*T*frag bytes. */
+/* block_ids: HOST array of n ids.  packed: DEVICE (or device-mapped / peer) buffer of n*T*frag bytes.
+ * A pool may be used from several host threads at once, each on its own stream: the host id lists of concurrent
+ * calls (these two and kvb_migrate_blocks) go through separate scratch slots. */
 int kvb_gather_blocks(kvb_pool_t* pool, const int64_t* block_ids, int64_t n, void* packed, void* stream, int flags);
 int kvb_scatter_blocks(kvb_pool_t* pool, const int64_t* block_ids, int64_t n, const void* packed, void* stream,
                        int flags);

@@ -7,6 +7,7 @@
 #include <cstdint>
 #include <cstdio>
 #include <exception>
+#include <mutex>
 #include <new>
 #include <string>
 #include <vector>
@@ -105,7 +106,9 @@ struct kvb_pool {
     cudaEvent_t free_ev = nullptr;
   } id_slots[kIdSlots];
   int next_slot = 0;
-  cudaEvent_t last_ids_ev = nullptr;  // event of the slot handed out by the latest upload_ids()
+  // held by a host-id call from taking its slot until it has recorded the slot's event: calls from several host
+  // threads must neither share a slot nor let the ring come round to a slot before its release is recorded
+  std::mutex ids_mu;
 };
 
 namespace kvb {
@@ -117,8 +120,10 @@ int launch_scatter(const kvb_pool* pool, const int64_t* ids_dev, int64_t n, cons
 int launch_migrate(const kvb_pool* src, const kvb_pool* dst, const int64_t* src_ids_dev, const int64_t* dst_ids_dev,
                    int64_t n, cudaStream_t s, int flags);
 // copies ids into a free scratch slot and enqueues the H2D on s; after launching the kernel that reads *out_dev the
-// caller records pool->last_ids_ev on s (release of the slot)
-int upload_ids(kvb_pool* pool, const int64_t* ids_host, int64_t n, cudaStream_t s, const int64_t** out_dev);
+// caller records *done_ev on s (release of the slot).  The caller holds pool->ids_mu from before this call until that
+// record.
+int upload_ids(kvb_pool* pool, const int64_t* ids_host, int64_t n, cudaStream_t s, const int64_t** out_dev,
+               cudaEvent_t* done_ev);
 int validate_ids(const kvb_pool* pool, const int64_t* ids_host, int64_t n);
 
 // hashing (device-resident arguments)

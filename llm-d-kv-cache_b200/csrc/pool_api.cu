@@ -54,7 +54,8 @@ int validate_ids(const kvb_pool* pool, const int64_t* ids, int64_t n) {
 }
 
 // Upload ids through one slot of the pool's scratch ring (see kvb_internal.h).
-int upload_ids(kvb_pool* pool, const int64_t* ids_host, int64_t n, cudaStream_t s, const int64_t** out_dev) {
+int upload_ids(kvb_pool* pool, const int64_t* ids_host, int64_t n, cudaStream_t s, const int64_t** out_dev,
+               cudaEvent_t* done_ev) {
   kvb_pool::IdSlot& sl = pool->id_slots[pool->next_slot];
   pool->next_slot = (pool->next_slot + 1) % kvb_pool::kIdSlots;
   if (!sl.free_ev) KVB_CUDA_TRY(cudaEventCreateWithFlags(&sl.free_ev, cudaEventDisableTiming));
@@ -75,7 +76,7 @@ int upload_ids(kvb_pool* pool, const int64_t* ids_host, int64_t n, cudaStream_t 
   std::memcpy(sl.h_ids, ids_host, n * sizeof(int64_t));
   KVB_CUDA_TRY(cudaMemcpyAsync(sl.d_ids, sl.h_ids, n * sizeof(int64_t), cudaMemcpyHostToDevice, s));
   *out_dev = sl.d_ids;
-  pool->last_ids_ev = sl.free_ev;
+  *done_ev = sl.free_ev;
   return KVB_OK;
 }
 
@@ -281,10 +282,12 @@ static int gs_host(kvb_pool_t* pool, const int64_t* ids, int64_t n, void* packed
   DeviceGuard g(pool->device);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   const int64_t* d = nullptr;
-  rc = upload_ids(pool, ids, n, s, &d);
+  cudaEvent_t done = nullptr;
+  std::lock_guard<std::mutex> lk(pool->ids_mu);
+  rc = upload_ids(pool, ids, n, s, &d, &done);
   if (rc) return rc;
   rc = gather ? launch_gather(pool, d, n, packed, s, flags) : launch_scatter(pool, d, n, packed, s, flags);
-  cudaEventRecord(pool->last_ids_ev, s);
+  cudaEventRecord(done, s);
   return rc;
 }
 
@@ -508,10 +511,12 @@ int kvb_migrate_blocks(kvb_pool_t* src, kvb_pool_t* dst, const int64_t* src_ids,
     std::memcpy(both.data(), src_ids, n * sizeof(int64_t));
     std::memcpy(both.data() + n, dst_ids, n * sizeof(int64_t));
     const int64_t* d = nullptr;
-    rc = upload_ids(src, both.data(), 2 * n, s, &d);
+    cudaEvent_t done = nullptr;
+    std::lock_guard<std::mutex> lk(src->ids_mu);
+    rc = upload_ids(src, both.data(), 2 * n, s, &d, &done);
     if (rc) return rc;
     rc = launch_migrate(src, dst, d, d + n, n, s, flags);
-    cudaEventRecord(src->last_ids_ev, s);
+    cudaEventRecord(done, s);
     return rc;
   });
 }
