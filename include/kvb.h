@@ -343,6 +343,36 @@ int kvb_enable_peer_access(int device, int peer_device);
 int kvb_migrate_blocks(kvb_pool_t* src, kvb_pool_t* dst, const int64_t* src_ids, const int64_t* dst_ids, int64_t n,
                        void* stream, int flags);
 
+/* KV geometry: how one fragment holds the KV heads of one block, for migration between pools of different
+ * tensor-parallel size or head layout (a prefill pool at TP=1 feeding decode ranks at TP=2, FlashAttention's NHD
+ * feeding FlashInfer's HND).
+ *   planes      1 when K and V are separate canonical tensors, 2 when K and V share a fragment
+ *   tokens      B, tokens per block
+ *   heads       H, the KV heads this pool holds (an MLA latent is one head)
+ *   head_bytes  E = head_size x element size
+ *   layout      KVB_KV_LAYOUT_NHD: byte (p, t, h, e) at ((p*B + t)*H + h)*E + e
+ *               KVB_KV_LAYOUT_HND: byte (p, t, h, e) at ((p*H + h)*B + t)*E + e
+ * A geometry is valid when every field is >= 1 and planes*tokens*heads*head_bytes == frag_bytes (< 4 GiB). */
+#define KVB_KV_LAYOUT_NHD 0
+#define KVB_KV_LAYOUT_HND 1
+typedef struct kvb_kv_geometry {
+  int32_t planes, tokens, heads, head_bytes, layout, pad;
+} kvb_kv_geometry_t;
+int kvb_pool_set_geometry(kvb_pool_t* pool, const kvb_kv_geometry_t* geom);
+
+/* Head-slice migration.  For every i < n, tensor k, plane p, token t, byte e and j < n_heads:
+ *   dst.tensor[k][dst_ids[i]*dst_stride + off_dst(p, t, dst_head0 + j, e)]
+ *     = src.tensor[k][src_ids[i]*src_stride + off_src(p, t, src_head0 + j, e)]
+ * and nothing else in the destination is written, so several source pools can each fill their own heads of one
+ * destination block.  Both pools need a geometry with equal tensor count, planes, tokens and head_bytes; both head
+ * ranges must lie in [0, heads) of their pool; the pools must be described on one device (a peer destination is
+ * described on the source device, as for kvb_migrate_blocks).  Any violation, or an id out of range, returns
+ * KVB_ERR_INVALID before anything is uploaded or launched.  n == 0 launches nothing.  Destination ids within one call
+ * are distinct.  The whole fragment in the same layout runs kvb_migrate_blocks' mover with these flags; every other
+ * slice runs the head-slice vector mover, which reads flags bits 8-11 (unroll 2/4/8) and 12-19 (CTAs per SM). */
+int kvb_migrate_heads(kvb_pool_t* src, kvb_pool_t* dst, const int64_t* src_ids, const int64_t* dst_ids, int64_t n,
+                      int32_t src_head0, int32_t dst_head0, int32_t n_heads, void* stream, int flags);
+
 #ifdef __cplusplus
 }
 #endif

@@ -64,6 +64,13 @@ class IpcMem(C.Structure):
     _fields_ = [("handle", C.c_uint8 * 64), ("offset", C.c_int64)]
 
 
+KV_LAYOUT_NHD, KV_LAYOUT_HND = 0, 1
+
+
+class KvGeometry(C.Structure):  # kvb_kv_geometry_t
+    _fields_ = [(n, C.c_int32) for n in ("planes", "tokens", "heads", "head_bytes", "layout", "pad")]
+
+
 _vp, _i32, _i64, _u64 = C.c_void_p, C.c_int32, C.c_int64, C.c_uint64
 _P = C.POINTER
 
@@ -120,6 +127,8 @@ SIGNATURES = {
     "kvb_ipc_close": (C.c_int, [C.c_int, _vp, _i64]),
     "kvb_enable_peer_access": (C.c_int, [C.c_int, C.c_int]),
     "kvb_migrate_blocks": (C.c_int, [_vp, _vp, _P(_i64), _P(_i64), _i64, _vp, C.c_int]),
+    "kvb_pool_set_geometry": (C.c_int, [_vp, _P(KvGeometry)]),
+    "kvb_migrate_heads": (C.c_int, [_vp, _vp, _P(_i64), _P(_i64), _i64, _i32, _i32, _i32, _vp, C.c_int]),
 }
 
 _lib = None

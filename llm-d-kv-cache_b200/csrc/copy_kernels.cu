@@ -304,6 +304,90 @@ static cudaError_t launch_ldg(CopyArgs a, int vec, int device, cudaStream_t s, i
   }
 }
 
+// ------------------------------------------------------------------------------------------
+// head-slice mover (kvb_migrate_heads): heads [hs0, hs0+nh) of every source fragment -> heads [hd0, hd0+nh) of the
+// destination fragment, each side in its own layout (kvb.h section 5 gives the offset formulas)
+// ------------------------------------------------------------------------------------------
+struct HeadArgs {
+  const uint8_t* const* src_t;
+  const uint8_t* const* dst_t;
+  const int64_t* src_ids;
+  const int64_t* dst_ids;
+  int64_t src_stride, dst_stride;
+  uint32_t T, P, B, E;
+  uint32_t Hs, Hd, hs0, hd0, nh;
+  uint32_t src_hnd, dst_hnd;
+  uint32_t run_kind;   // 0: NHD->NHD, 1: HND->HND, 2: mixed (runs in the destination's order)
+  uint32_t run_bytes;  // nh*E, nh*B*E or E
+  uint32_t pair_bytes; // P*B*nh*E: what one (block, tensor) pair moves
+  uint32_t ppp;        // pieces per pair
+  uint32_t piece;      // bytes per piece (the last piece of a pair may be shorter)
+  uint64_t total_items;
+};
+
+__device__ __forceinline__ uint32_t kv_off(uint32_t hnd, uint32_t p, uint32_t t, uint32_t h, uint32_t H, uint32_t B,
+                                           uint32_t E) {
+  return hnd ? ((p * H + h) * B + t) * E : ((p * B + t) * H + h) * E;
+}
+
+template <typename V, int UNROLL>
+__global__ void __launch_bounds__(kLdgThreads) paged_copy_heads_kernel(const HeadArgs a) {
+  for (uint64_t item = blockIdx.x; item < a.total_items; item += gridDim.x) {
+    const uint64_t pair = item / a.ppp;
+    const uint32_t pc = (uint32_t)(item - pair * a.ppp);
+    const uint64_t blk = pair / a.T;
+    const uint32_t k = (uint32_t)(pair - blk * a.T);
+    const uint8_t* sfrag = ldg_ptr(a.src_t + k) + __ldg(a.src_ids + blk) * a.src_stride;
+    uint8_t* dfrag = const_cast<uint8_t*>(ldg_ptr(a.dst_t + k)) + __ldg(a.dst_ids + blk) * a.dst_stride;
+    const uint32_t q0 = pc * a.piece;
+    const uint32_t end = min(a.pair_bytes, q0 + a.piece);
+    for (uint32_t base = q0; base < end; base += kLdgThreads * UNROLL * (uint32_t)sizeof(V)) {
+      V v[UNROLL];
+      uint32_t doff[UNROLL];
+#pragma unroll
+      for (int u = 0; u < UNROLL; ++u) {
+        const uint32_t q = base + (threadIdx.x + u * kLdgThreads) * (uint32_t)sizeof(V);
+        if (q < end) {
+          // byte q of the pair -> (run, offset in run) -> (plane, token, head j of the slice)
+          const uint32_t r = q / a.run_bytes, o = q - r * a.run_bytes;
+          uint32_t p, t, j;
+          if (a.run_kind == 0) {
+            p = r / a.B, t = r - p * a.B, j = 0;
+          } else if (a.run_kind == 1) {
+            p = r, t = 0, j = 0;
+          } else if (a.dst_hnd) {  // runs (p, j, t), t fastest
+            t = r % a.B;
+            const uint32_t r2 = r / a.B;
+            j = r2 % a.nh, p = r2 / a.nh;
+          } else {  // runs (p, t, j), j fastest
+            j = r % a.nh;
+            const uint32_t r2 = r / a.nh;
+            t = r2 % a.B, p = r2 / a.B;
+          }
+          const uint32_t soff = kv_off(a.src_hnd, p, t, a.hs0 + j, a.Hs, a.B, a.E) + o;
+          doff[u] = kv_off(a.dst_hnd, p, t, a.hd0 + j, a.Hd, a.B, a.E) + o;
+          v[u] = ld_any<V>(reinterpret_cast<const V*>(sfrag + soff));
+        }
+      }
+#pragma unroll
+      for (int u = 0; u < UNROLL; ++u) {
+        const uint32_t q = base + (threadIdx.x + u * kLdgThreads) * (uint32_t)sizeof(V);
+        if (q < end) st_any<V>(reinterpret_cast<V*>(dfrag + doff[u]), v[u]);
+      }
+    }
+  }
+}
+
+template <typename V>
+static cudaError_t launch_heads_v(const HeadArgs& a, int grid, int unroll, cudaStream_t s) {
+  switch (unroll) {
+    case 2: paged_copy_heads_kernel<V, 2><<<grid, kLdgThreads, 0, s>>>(a); break;
+    case 8: paged_copy_heads_kernel<V, 8><<<grid, kLdgThreads, 0, s>>>(a); break;
+    default: paged_copy_heads_kernel<V, 4><<<grid, kLdgThreads, 0, s>>>(a); break;
+  }
+  return cudaGetLastError();
+}
+
 template <int MODE, int STAGES, int LOOKAHEAD>
 static cudaError_t launch_bulk_cfg(const CopyArgs& a, int grid, size_t smem, cudaStream_t s) {
   auto k = paged_copy_bulk_kernel<MODE, STAGES, LOOKAHEAD>;
@@ -404,6 +488,64 @@ int launch_migrate(const kvb_pool* src, const kvb_pool* dst, const int64_t* src_
   // than the bulk ring's shared memory.  Not yet swept on H100 (tools/tune_migrate.py needs two GPUs); local HBM keeps bulk
   if ((flags & 0xff) == KVB_COPY_DEFAULT && dst->peer && vec == 16) flags = KVB_COPY_LDG | (4 << 8) | (8 << 12);
   return launch_copy<kMigrate>(a, vec, src->device, s, flags);
+}
+
+int launch_migrate_heads(const kvb_pool* src, const kvb_pool* dst, const int64_t* src_ids_dev,
+                         const int64_t* dst_ids_dev, int64_t n, int src_head0, int dst_head0, int n_heads,
+                         cudaStream_t s, int flags) {
+  const kvb_kv_geometry_t& gs = src->geom;
+  const kvb_kv_geometry_t& gd = dst->geom;
+  // the whole fragment in the same layout is a plain page copy: the migrate mover takes it
+  if (n_heads == gs.heads && n_heads == gd.heads && src_head0 == 0 && dst_head0 == 0 && gs.layout == gd.layout)
+    return launch_migrate(src, dst, src_ids_dev, dst_ids_dev, n, s, flags);
+  if (n == 0) return KVB_OK;
+  HeadArgs a{};
+  a.src_t = src->d_tensor_ptrs;
+  a.dst_t = dst->d_tensor_ptrs;
+  a.src_ids = src_ids_dev;
+  a.dst_ids = dst_ids_dev;
+  a.src_stride = src->stride_bytes;
+  a.dst_stride = dst->stride_bytes;
+  a.T = (uint32_t)src->num_tensors;
+  a.P = (uint32_t)gs.planes;
+  a.B = (uint32_t)gs.tokens;
+  a.E = (uint32_t)gs.head_bytes;
+  a.Hs = (uint32_t)gs.heads;
+  a.Hd = (uint32_t)gd.heads;
+  a.hs0 = (uint32_t)src_head0;
+  a.hd0 = (uint32_t)dst_head0;
+  a.nh = (uint32_t)n_heads;
+  a.src_hnd = gs.layout == KVB_KV_LAYOUT_HND;
+  a.dst_hnd = gd.layout == KVB_KV_LAYOUT_HND;
+  a.run_kind = gs.layout != gd.layout ? 2 : (a.src_hnd ? 1 : 0);
+  a.run_bytes = a.run_kind == 0 ? a.nh * a.E : (a.run_kind == 1 ? a.nh * a.B * a.E : a.E);
+  a.pair_bytes = a.P * a.B * a.nh * a.E;
+  // every run starts at a multiple of E on both sides: the vector may be as wide as E's largest power-of-two factor
+  int vec = std::min(src->vec_bytes, dst->vec_bytes);
+  while (vec > 1 && (a.E % vec)) vec >>= 1;
+  if (vec < 4) vec = 1;
+  Tuning t = tuning();
+  if ((flags >> 8) & 0xf) t.ldg_unroll = (flags >> 8) & 0xf;
+  if ((flags >> 12) & 0xff) t.ldg_ctas_per_sm = (flags >> 12) & 0xff;
+  const int unroll = (t.ldg_unroll == 2 || t.ldg_unroll == 8) ? t.ldg_unroll : 4;
+  a.piece = (uint32_t)(kLdgThreads * unroll * vec);
+  a.ppp = (a.pair_bytes + a.piece - 1) / a.piece;
+  a.total_items = (uint64_t)n * a.T * a.ppp;
+  const uint64_t cap = (uint64_t)sm_count(src->device) * (uint64_t)std::max(1, t.ldg_ctas_per_sm);
+  const int grid = (int)std::max<uint64_t>(1, std::min<uint64_t>(a.total_items, cap));
+  cudaError_t e;
+  switch (vec) {
+    case 16: e = launch_heads_v<int4>(a, grid, unroll, s); break;
+    case 8: e = launch_heads_v<uint2>(a, grid, unroll, s); break;
+    case 4: e = launch_heads_v<uint32_t>(a, grid, unroll, s); break;
+    default: e = launch_heads_v<uint8_t>(a, grid, unroll, s); break;
+  }
+  if (e != cudaSuccess) {
+    set_error("head-slice migrate launch failed: %s", cudaGetErrorString(e));
+    return KVB_ERR_CUDA;
+  }
+  count_launch();
+  return KVB_OK;
 }
 
 }  // namespace kvb

@@ -109,6 +109,9 @@ struct kvb_pool {
   // held by a host-id call from taking its slot until it has recorded the slot's event: calls from several host
   // threads must neither share a slot nor let the ring come round to a slot before its release is recorded
   std::mutex ids_mu;
+  // how each fragment holds its KV heads (kvb_pool_set_geometry); kvb_migrate_heads refuses pools without one
+  bool has_geom = false;
+  kvb_kv_geometry_t geom{};
 };
 
 namespace kvb {
@@ -119,6 +122,11 @@ int launch_scatter(const kvb_pool* pool, const int64_t* ids_dev, int64_t n, cons
                    int flags);
 int launch_migrate(const kvb_pool* src, const kvb_pool* dst, const int64_t* src_ids_dev, const int64_t* dst_ids_dev,
                    int64_t n, cudaStream_t s, int flags);
+// heads [src_head0, +n_heads) of src's fragments -> heads [dst_head0, +n_heads) of dst's (both pools carry a geometry,
+// arguments already checked); the whole fragment in the same layout goes to launch_migrate
+int launch_migrate_heads(const kvb_pool* src, const kvb_pool* dst, const int64_t* src_ids_dev,
+                         const int64_t* dst_ids_dev, int64_t n, int src_head0, int dst_head0, int n_heads,
+                         cudaStream_t s, int flags);
 // copies ids into a free scratch slot and enqueues the H2D on s; after launching the kernel that reads *out_dev the
 // caller records *done_ev on s (release of the slot).  The caller holds pool->ids_mu from before this call until that
 // record.

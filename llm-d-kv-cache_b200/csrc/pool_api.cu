@@ -521,4 +521,64 @@ int kvb_migrate_blocks(kvb_pool_t* src, kvb_pool_t* dst, const int64_t* src_ids,
   });
 }
 
+int kvb_pool_set_geometry(kvb_pool_t* p, const kvb_kv_geometry_t* g) {
+  return kvb::guarded([&]() -> int {
+    KVB_REQUIRE(p && g, "NULL argument");
+    KVB_REQUIRE(g->planes >= 1 && g->tokens >= 1 && g->heads >= 1 && g->head_bytes >= 1,
+                "geometry: planes, tokens, heads and head_bytes must be >= 1 (got %d, %d, %d, %d)", g->planes,
+                g->tokens, g->heads, g->head_bytes);
+    KVB_REQUIRE(g->layout == KVB_KV_LAYOUT_NHD || g->layout == KVB_KV_LAYOUT_HND, "geometry: unknown layout %d",
+                g->layout);
+    const int64_t bytes = (int64_t)g->planes * g->tokens * g->heads * g->head_bytes;
+    KVB_REQUIRE(bytes == p->frag_bytes, "geometry: planes x tokens x heads x head_bytes = %lld, fragment is %lld B",
+                (long long)bytes, (long long)p->frag_bytes);
+    KVB_REQUIRE(bytes <= 0xffffffffll, "geometry: fragments of 4 GiB or more are not supported");
+    p->geom = *g;
+    p->geom.pad = 0;
+    p->has_geom = true;
+    return KVB_OK;
+  });
+}
+
+int kvb_migrate_heads(kvb_pool_t* src, kvb_pool_t* dst, const int64_t* src_ids, const int64_t* dst_ids, int64_t n,
+                      int32_t src_head0, int32_t dst_head0, int32_t n_heads, void* stream, int flags) {
+  return kvb::guarded([&]() -> int {
+    KVB_REQUIRE(src && dst, "pool is NULL");
+    KVB_REQUIRE(n >= 0, "negative block count");
+    KVB_REQUIRE(src->has_geom && dst->has_geom, "migrate_heads: the %s pool has no KV geometry",
+                src->has_geom ? "destination" : "source");
+    const kvb_kv_geometry_t &gs = src->geom, &gd = dst->geom;
+    KVB_REQUIRE(src->num_tensors == dst->num_tensors && gs.planes == gd.planes && gs.tokens == gd.tokens &&
+                    gs.head_bytes == gd.head_bytes,
+                "migrate_heads: pools differ in shape (T %d vs %d, planes %d vs %d, tokens %d vs %d, head_bytes %d vs %d)",
+                src->num_tensors, dst->num_tensors, gs.planes, gd.planes, gs.tokens, gd.tokens, gs.head_bytes,
+                gd.head_bytes);
+    KVB_REQUIRE(n_heads >= 1 && src_head0 >= 0 && dst_head0 >= 0 && (int64_t)src_head0 + n_heads <= gs.heads &&
+                    (int64_t)dst_head0 + n_heads <= gd.heads,
+                "migrate_heads: heads [%d, +%d) -> [%d, +%d) out of range (source holds %d, destination %d)", src_head0,
+                n_heads, dst_head0, n_heads, gs.heads, gd.heads);
+    KVB_REQUIRE(dst->device == src->device,
+                "migrate_heads: describe the destination pool on the source device (peer/IPC pointers)");
+    if (n == 0) return KVB_OK;
+    KVB_REQUIRE(src_ids && dst_ids, "ids NULL");
+    int rc = validate_ids(src, src_ids, n);
+    if (rc) return rc;
+    rc = validate_ids(dst, dst_ids, n);
+    if (rc) return rc;
+    DeviceGuard g(src->device);
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    std::vector<int64_t> both(2 * n);  // one scratch upload: [src ids | dst ids]
+    std::memcpy(both.data(), src_ids, n * sizeof(int64_t));
+    std::memcpy(both.data() + n, dst_ids, n * sizeof(int64_t));
+    const int64_t* d = nullptr;
+    cudaEvent_t done = nullptr;
+    std::lock_guard<std::mutex> lk(src->ids_mu);
+    rc = upload_ids(src, both.data(), 2 * n, s, &d, &done);
+    if (rc) return rc;
+    rc = launch_migrate_heads(src, dst, d, d + n, n, src_head0, dst_head0, n_heads, s, flags);
+    cudaEventRecord(done, s);
+    return rc;
+  });
+}
+
 }  // extern "C"

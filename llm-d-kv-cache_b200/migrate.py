@@ -24,7 +24,10 @@ def export_pool(pool: KVPool) -> dict:
         m = IpcMem()
         check(lib.kvb_ipc_export(pool.device, t.data_ptr(), C.byref(m)))
         mems.append((bytes(m.handle), int(m.offset)))
-    return {"device": pool.device, "num_blocks": pool.num_blocks, "frag_bytes": pool.frag_bytes, "mems": mems}
+    desc = {"device": pool.device, "num_blocks": pool.num_blocks, "frag_bytes": pool.frag_bytes, "mems": mems}
+    if pool.geometry is not None:
+        desc["geometry"] = tuple(pool.geometry)
+    return desc
 
 
 class RemotePool(KVPool):
@@ -47,7 +50,7 @@ class RemotePool(KVPool):
                 self._imported.append(base)
             ptrs.append(base + offset)
         super().__init__(None, local_device, ptrs=ptrs, num_blocks=desc["num_blocks"],
-                         frag_bytes=desc["frag_bytes"], stride_bytes=desc["frag_bytes"])
+                         frag_bytes=desc["frag_bytes"], stride_bytes=desc["frag_bytes"], geometry=desc.get("geometry"))
         check(lib.kvb_pool_mark_peer(self.handle, 1))
 
     def close(self):
@@ -65,6 +68,19 @@ def migrate_blocks(src: KVPool, dst: KVPool, src_ids: Sequence[int], dst_ids: Se
         raise ValueError("src_ids and dst_ids differ in length")
     check(_lib.load().kvb_migrate_blocks(src.handle, dst.handle, s.ctypes.data_as(C.POINTER(C.c_int64)),
                                          d.ctypes.data_as(C.POINTER(C.c_int64)), s.size, _stream_ptr(stream), flags))
+
+
+def migrate_heads(src: KVPool, dst: KVPool, src_ids: Sequence[int], dst_ids: Sequence[int], src_head0: int,
+                  dst_head0: int, n_heads: int, stream=None, flags: int = 0) -> None:
+    """Heads [src_head0, src_head0 + n_heads) of src pages src_ids[i] -> heads [dst_head0, dst_head0 + n_heads) of dst
+    pages dst_ids[i], each pool in its own KV geometry (kvb.h section 5); the rest of each destination page is left
+    alone.  Both pools need a geometry; partition.tp_head_transfers plans the calls of a TP resharding."""
+    s, d = _ids_array(src_ids), _ids_array(dst_ids)
+    if s.size != d.size:
+        raise ValueError("src_ids and dst_ids differ in length")
+    check(_lib.load().kvb_migrate_heads(src.handle, dst.handle, s.ctypes.data_as(C.POINTER(C.c_int64)),
+                                        d.ctypes.data_as(C.POINTER(C.c_int64)), s.size, int(src_head0),
+                                        int(dst_head0), int(n_heads), _stream_ptr(stream), flags))
 
 
 def enable_peer_access(device: int, peer: int) -> None:

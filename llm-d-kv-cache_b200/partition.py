@@ -32,6 +32,47 @@ def fanout_plan(n_blocks: int, world: int, root: int = 0) -> dict:
     return {p: (i * n_blocks, (i + 1) * n_blocks) for i, p in enumerate(peers)}
 
 
+def _kv_heads_of(rank: int, tp: int, num_kv_heads: int, mla: bool) -> range:
+    """Global KV heads a TP rank holds (vLLM's rule): a contiguous H/tp share when tp <= H, one head replicated on
+    tp/H ranks when tp > H, the one latent head everywhere for MLA."""
+    if mla:
+        return range(0, 1)
+    if tp <= num_kv_heads:
+        if num_kv_heads % tp:
+            raise ValueError(f"{num_kv_heads} KV heads do not split over TP={tp}")
+        per = num_kv_heads // tp
+        return range(rank * per, (rank + 1) * per)
+    if tp % num_kv_heads:
+        raise ValueError(f"TP={tp} is not a multiple of {num_kv_heads} KV heads")
+    h = rank // (tp // num_kv_heads)
+    return range(h, h + 1)
+
+
+def tp_head_transfers(num_kv_heads: int, src_tp: int, dst_tp: int, mla: bool = False) -> list:
+    """KV hand-off plan between a TP=src_tp pool set and a TP=dst_tp pool set of one model:
+    [(src_rank, dst_rank, src_head0, dst_head0, n_heads)], head indices local to each rank's pool, one
+    migrate.migrate_heads call each.  Every destination head is written exactly once; where several source ranks hold
+    it (replicated heads), destination rank d reads from holders[d % len(holders)].  Consecutive heads from one source
+    rank are merged into one transfer."""
+    if num_kv_heads < 1 or src_tp < 1 or dst_tp < 1:
+        raise ValueError("num_kv_heads and TP sizes must be >= 1")
+    H = 1 if mla else num_kv_heads
+    src_heads = [_kv_heads_of(r, src_tp, H, mla) for r in range(src_tp)]
+    out = []
+    for d in range(dst_tp):
+        mine = _kv_heads_of(d, dst_tp, H, mla)
+        for j, h in enumerate(mine):
+            holders = [r for r in range(src_tp) if h in src_heads[r]]
+            s = holders[d % len(holders)]
+            sh = h - src_heads[s].start
+            last = out[-1] if out else None
+            if last and last[0] == s and last[1] == d and last[2] + last[4] == sh and last[3] + last[4] == j:
+                out[-1] = (s, d, last[2], last[3], last[4] + 1)
+            else:
+                out.append((s, d, sh, j, 1))
+    return out
+
+
 def exchange_objects(obj, dist=None) -> list:
     """all_gather of one picklable object per rank (pool descriptors, checksums)."""
     if dist is None or not dist.is_initialized() or dist.get_world_size() == 1:

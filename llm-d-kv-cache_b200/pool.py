@@ -2,7 +2,7 @@
 from __future__ import annotations
 
 import ctypes as C
-from typing import Sequence
+from typing import NamedTuple, Sequence
 
 import numpy as np
 
@@ -23,12 +23,27 @@ def _ids_array(block_ids) -> np.ndarray:
     return np.ascontiguousarray(np.asarray(block_ids, dtype=np.int64).reshape(-1))
 
 
+_LAYOUTS = {"NHD": _lib.KV_LAYOUT_NHD, "HND": _lib.KV_LAYOUT_HND}
+
+
+class KVGeometry(NamedTuple):
+    """How one fragment holds the KV heads of a block (kvb.h section 5).  planes: 1 when K and V are separate
+    tensors, 2 when they share a fragment; tokens: block size; heads: the KV heads this pool holds; head_bytes:
+    head_size x element size; layout: "NHD" ([token][head][byte]) or "HND" ([head][token][byte])."""
+    planes: int
+    tokens: int
+    heads: int
+    head_bytes: int
+    layout: str = "NHD"
+
+
 class KVPool:
     """Borrowed view of the KV cache: list of CUDA tensors, each (num_blocks, page_size_bytes)
-    (reference: TensorCopier ctor, csrc/storage/tensor_copier.cu:31-48)."""
+    (reference: TensorCopier ctor, csrc/storage/tensor_copier.cu:31-48).  ``geometry`` (a KVGeometry) lets the pool
+    take part in head-slice migration (migrate.migrate_heads)."""
 
     def __init__(self, tensors: Sequence, device: int | None = None, *, ptrs=None, num_blocks=None,
-                 frag_bytes=None, stride_bytes=None):
+                 frag_bytes=None, stride_bytes=None, geometry=None):
         lib = _lib.load()
         if ptrs is None:
             if not tensors:
@@ -55,6 +70,18 @@ class KVPool:
         check(lib.kvb_pool_create(self.device, arr, len(ptrs), self.num_blocks, self.frag_bytes,
                                   int(stride_bytes), C.byref(h)))
         self.handle = h
+        self.geometry = None
+        if geometry is not None:
+            self.set_geometry(geometry)
+
+    def set_geometry(self, geometry) -> None:
+        """Declare how each fragment holds its KV heads; planes x tokens x heads x head_bytes must be the fragment."""
+        g = KVGeometry(*geometry)
+        if g.layout not in _LAYOUTS:
+            raise ValueError(f"layout must be 'NHD' or 'HND', not {g.layout!r}")
+        c = _lib.KvGeometry(int(g.planes), int(g.tokens), int(g.heads), int(g.head_bytes), _LAYOUTS[g.layout], 0)
+        check(_lib.load().kvb_pool_set_geometry(self.handle, C.byref(c)))
+        self.geometry = g
 
     def close(self):
         if getattr(self, "handle", None):
