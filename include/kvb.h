@@ -373,6 +373,28 @@ int kvb_pool_set_geometry(kvb_pool_t* pool, const kvb_kv_geometry_t* geom);
 int kvb_migrate_heads(kvb_pool_t* src, kvb_pool_t* dst, const int64_t* src_ids, const int64_t* dst_ids, int64_t n,
                       int32_t src_head0, int32_t dst_head0, int32_t n_heads, void* stream, int flags);
 
+/* Token-segment migration, for pools of different block sizes (a 16-token prefill pool feeding a 64-token decode
+ * pool) and for transfers that start part-way into a block (the decode side already holds a cached prefix).
+ * A segment is a run of n_tokens consecutive token slots of one source block and one destination block. */
+typedef struct kvb_token_segment {
+  int64_t src_block, dst_block;
+  int32_t src_tok0, dst_tok0, n_tokens, pad;
+} kvb_token_segment_t; /* 32 B */
+/* For every segment s, tensor k, plane p, i < s.n_tokens, j < n_heads and byte e:
+ *   dst.tensor[k][s.dst_block*dst_stride + off_dst(p, s.dst_tok0 + i, dst_head0 + j, e)]
+ *     = src.tensor[k][s.src_block*src_stride + off_src(p, s.src_tok0 + i, src_head0 + j, e)]
+ * and nothing else in the destination is written.  Each side uses its own geometry's tokens (B), heads and layout in
+ * the offset formulas above.  Both pools need a geometry; tensor count, planes and head_bytes must be equal, tokens,
+ * heads and layout may differ.  KVB_ERR_INVALID, before anything is uploaded or launched, for: a NULL pool or
+ * n_segs < 0; a pool without a geometry; a shape mismatch; a head range outside [0, heads) of its pool; pools
+ * described on different devices; a segment with n_tokens < 1, a tok0 < 0 or tok0 + n_tokens > B of its side; a block
+ * id outside its pool; two segments whose destination token ranges in one block overlap.  n_segs == 0 launches
+ * nothing.  When every segment covers whole blocks on both sides (tok0 == 0, n_tokens == B of both pools) the call
+ * runs exactly what kvb_migrate_heads runs on the two id lists; otherwise the token-segment vector mover, which reads
+ * flags bits 8-11 (unroll 2/4/8) and 12-19 (CTAs per SM). */
+int kvb_migrate_tokens(kvb_pool_t* src, kvb_pool_t* dst, const kvb_token_segment_t* segs, int64_t n_segs,
+                       int32_t src_head0, int32_t dst_head0, int32_t n_heads, void* stream, int flags);
+
 #ifdef __cplusplus
 }
 #endif

@@ -71,6 +71,11 @@ class KvGeometry(C.Structure):  # kvb_kv_geometry_t
     _fields_ = [(n, C.c_int32) for n in ("planes", "tokens", "heads", "head_bytes", "layout", "pad")]
 
 
+class TokenSegment(C.Structure):  # kvb_token_segment_t
+    _fields_ = [("src_block", C.c_int64), ("dst_block", C.c_int64), ("src_tok0", C.c_int32), ("dst_tok0", C.c_int32),
+                ("n_tokens", C.c_int32), ("pad", C.c_int32)]
+
+
 _vp, _i32, _i64, _u64 = C.c_void_p, C.c_int32, C.c_int64, C.c_uint64
 _P = C.POINTER
 
@@ -129,6 +134,7 @@ SIGNATURES = {
     "kvb_migrate_blocks": (C.c_int, [_vp, _vp, _P(_i64), _P(_i64), _i64, _vp, C.c_int]),
     "kvb_pool_set_geometry": (C.c_int, [_vp, _P(KvGeometry)]),
     "kvb_migrate_heads": (C.c_int, [_vp, _vp, _P(_i64), _P(_i64), _i64, _i32, _i32, _i32, _vp, C.c_int]),
+    "kvb_migrate_tokens": (C.c_int, [_vp, _vp, _P(TokenSegment), _i64, _i32, _i32, _i32, _vp, C.c_int]),
 }
 
 _lib = None

@@ -330,6 +330,27 @@ __device__ __forceinline__ uint32_t kv_off(uint32_t hnd, uint32_t p, uint32_t t,
   return hnd ? ((p * H + h) * B + t) * E : ((p * B + t) * H + h) * E;
 }
 
+// run r of a slice of P planes x n tokens x nh heads -> (plane p, token i, head j) of its first byte, relative to the
+// slice's first token and head.  run_kind 0 (NHD->NHD): runs (p, i) of nh heads; 1 (HND->HND): head_runs runs per
+// plane of n tokens, each of one head (head_runs = nh) or of all nh heads (head_runs = 1: whole blocks, where the heads
+// are adjacent); 2 (mixed): runs of one head in the destination's order
+__device__ __forceinline__ void run_start(uint32_t run_kind, uint32_t dst_hnd, uint32_t r, uint32_t n, uint32_t nh,
+                                          uint32_t head_runs, uint32_t& p, uint32_t& i, uint32_t& j) {
+  if (run_kind == 0) {
+    p = r / n, i = r - p * n, j = 0;
+  } else if (run_kind == 1) {
+    p = r / head_runs, j = r - p * head_runs, i = 0;
+  } else if (dst_hnd) {  // runs (p, j, i), i fastest
+    i = r % n;
+    const uint32_t r2 = r / n;
+    j = r2 % nh, p = r2 / nh;
+  } else {  // runs (p, i, j), j fastest
+    j = r % nh;
+    const uint32_t r2 = r / nh;
+    i = r2 % n, p = r2 / n;
+  }
+}
+
 template <typename V, int UNROLL>
 __global__ void __launch_bounds__(kLdgThreads) paged_copy_heads_kernel(const HeadArgs a) {
   for (uint64_t item = blockIdx.x; item < a.total_items; item += gridDim.x) {
@@ -351,19 +372,7 @@ __global__ void __launch_bounds__(kLdgThreads) paged_copy_heads_kernel(const Hea
           // byte q of the pair -> (run, offset in run) -> (plane, token, head j of the slice)
           const uint32_t r = q / a.run_bytes, o = q - r * a.run_bytes;
           uint32_t p, t, j;
-          if (a.run_kind == 0) {
-            p = r / a.B, t = r - p * a.B, j = 0;
-          } else if (a.run_kind == 1) {
-            p = r, t = 0, j = 0;
-          } else if (a.dst_hnd) {  // runs (p, j, t), t fastest
-            t = r % a.B;
-            const uint32_t r2 = r / a.B;
-            j = r2 % a.nh, p = r2 / a.nh;
-          } else {  // runs (p, t, j), j fastest
-            j = r % a.nh;
-            const uint32_t r2 = r / a.nh;
-            t = r2 % a.B, p = r2 / a.B;
-          }
+          run_start(a.run_kind, a.dst_hnd, r, a.B, a.nh, 1, p, t, j);
           const uint32_t soff = kv_off(a.src_hnd, p, t, a.hs0 + j, a.Hs, a.B, a.E) + o;
           doff[u] = kv_off(a.dst_hnd, p, t, a.hd0 + j, a.Hd, a.B, a.E) + o;
           v[u] = ld_any<V>(reinterpret_cast<const V*>(sfrag + soff));
@@ -386,6 +395,93 @@ static cudaError_t launch_heads_v(const HeadArgs& a, int grid, int unroll, cudaS
     default: paged_copy_heads_kernel<V, 4><<<grid, kLdgThreads, 0, s>>>(a); break;
   }
   return cudaGetLastError();
+}
+
+// ------------------------------------------------------------------------------------------
+// token-segment mover (kvb_migrate_tokens): tokens [src_tok0, +n) x heads [hs0, +nh) of a source block -> tokens
+// [dst_tok0, +n) x heads [hd0, +nh) of a destination block, each side with its own block size and layout
+// ------------------------------------------------------------------------------------------
+struct TokenArgs {
+  const uint8_t* const* src_t;
+  const uint8_t* const* dst_t;
+  const kvb_token_segment_t* segs;
+  int64_t src_stride, dst_stride;
+  uint32_t T, P, E;
+  uint32_t Bs, Bd, Hs, Hd, hs0, hd0, nh;
+  uint32_t src_hnd, dst_hnd;
+  uint32_t run_kind;   // as HeadArgs; runs of nh*E, n*E or E bytes, n the segment's own token count
+  uint32_t tok_bytes;  // nh*E: one token of the slice in one plane
+  uint32_t ppp;        // pieces per (segment, tensor) pair, from the call's longest segment
+  uint32_t piece;      // bytes per piece (the last piece of a pair may be shorter)
+  uint64_t total_items;
+};
+
+template <typename V, int UNROLL>
+__global__ void __launch_bounds__(kLdgThreads) paged_copy_tokens_kernel(const TokenArgs a) {
+  for (uint64_t item = blockIdx.x; item < a.total_items; item += gridDim.x) {
+    const uint64_t pair = item / a.ppp;
+    const uint32_t pc = (uint32_t)(item - pair * a.ppp);
+    const uint64_t sg = pair / a.T;
+    const uint32_t k = (uint32_t)(pair - sg * a.T);
+    const kvb_token_segment_t* seg = a.segs + sg;
+    const uint32_t n = (uint32_t)__ldg(&seg->n_tokens);
+    const uint32_t seg_bytes = a.P * n * a.tok_bytes;
+    const uint32_t q0 = pc * a.piece;
+    if (q0 >= seg_bytes) continue;  // a segment shorter than the call's longest has fewer pieces
+    const uint32_t end = min(seg_bytes, q0 + a.piece);
+    const uint32_t run_bytes = a.run_kind == 0 ? a.tok_bytes : (a.run_kind == 1 ? n * a.E : a.E);
+    const uint32_t st0 = (uint32_t)__ldg(&seg->src_tok0), dt0 = (uint32_t)__ldg(&seg->dst_tok0);
+    const uint8_t* sfrag = ldg_ptr(a.src_t + k) + __ldg(&seg->src_block) * a.src_stride;
+    uint8_t* dfrag = const_cast<uint8_t*>(ldg_ptr(a.dst_t + k)) + __ldg(&seg->dst_block) * a.dst_stride;
+    for (uint32_t base = q0; base < end; base += kLdgThreads * UNROLL * (uint32_t)sizeof(V)) {
+      V v[UNROLL];
+      uint32_t doff[UNROLL];
+#pragma unroll
+      for (int u = 0; u < UNROLL; ++u) {
+        const uint32_t q = base + (threadIdx.x + u * kLdgThreads) * (uint32_t)sizeof(V);
+        if (q < end) {
+          // byte q of the segment -> (run, offset in run) -> (plane, token i, head j of the slice)
+          const uint32_t r = q / run_bytes, o = q - r * run_bytes;
+          uint32_t p, i, j;
+          run_start(a.run_kind, a.dst_hnd, r, n, a.nh, a.nh, p, i, j);
+          const uint32_t soff = kv_off(a.src_hnd, p, st0 + i, a.hs0 + j, a.Hs, a.Bs, a.E) + o;
+          doff[u] = kv_off(a.dst_hnd, p, dt0 + i, a.hd0 + j, a.Hd, a.Bd, a.E) + o;
+          v[u] = ld_any<V>(reinterpret_cast<const V*>(sfrag + soff));
+        }
+      }
+#pragma unroll
+      for (int u = 0; u < UNROLL; ++u) {
+        const uint32_t q = base + (threadIdx.x + u * kLdgThreads) * (uint32_t)sizeof(V);
+        if (q < end) st_any<V>(reinterpret_cast<V*>(dfrag + doff[u]), v[u]);
+      }
+    }
+  }
+}
+
+template <typename V>
+static cudaError_t launch_tokens_v(const TokenArgs& a, int grid, int unroll, cudaStream_t s) {
+  switch (unroll) {
+    case 2: paged_copy_tokens_kernel<V, 2><<<grid, kLdgThreads, 0, s>>>(a); break;
+    case 8: paged_copy_tokens_kernel<V, 8><<<grid, kLdgThreads, 0, s>>>(a); break;
+    default: paged_copy_tokens_kernel<V, 4><<<grid, kLdgThreads, 0, s>>>(a); break;
+  }
+  return cudaGetLastError();
+}
+
+// vector width, unroll and CTAs per SM of the head-slice and token-segment movers
+struct SliceCfg {
+  int vec, unroll, ctas_per_sm;
+};
+static SliceCfg slice_cfg(const kvb_pool* src, const kvb_pool* dst, uint32_t E, int flags) {
+  // every run starts at a multiple of E on both sides: the vector may be as wide as E's largest power-of-two factor
+  int vec = std::min(src->vec_bytes, dst->vec_bytes);
+  while (vec > 1 && (E % vec)) vec >>= 1;
+  if (vec < 4) vec = 1;
+  Tuning t = tuning();
+  if ((flags >> 8) & 0xf) t.ldg_unroll = (flags >> 8) & 0xf;
+  if ((flags >> 12) & 0xff) t.ldg_ctas_per_sm = (flags >> 12) & 0xff;
+  const int unroll = (t.ldg_unroll == 2 || t.ldg_unroll == 8) ? t.ldg_unroll : 4;
+  return {vec, unroll, std::max(1, t.ldg_ctas_per_sm)};
 }
 
 template <int MODE, int STAGES, int LOOKAHEAD>
@@ -520,28 +616,68 @@ int launch_migrate_heads(const kvb_pool* src, const kvb_pool* dst, const int64_t
   a.run_kind = gs.layout != gd.layout ? 2 : (a.src_hnd ? 1 : 0);
   a.run_bytes = a.run_kind == 0 ? a.nh * a.E : (a.run_kind == 1 ? a.nh * a.B * a.E : a.E);
   a.pair_bytes = a.P * a.B * a.nh * a.E;
-  // every run starts at a multiple of E on both sides: the vector may be as wide as E's largest power-of-two factor
-  int vec = std::min(src->vec_bytes, dst->vec_bytes);
-  while (vec > 1 && (a.E % vec)) vec >>= 1;
-  if (vec < 4) vec = 1;
-  Tuning t = tuning();
-  if ((flags >> 8) & 0xf) t.ldg_unroll = (flags >> 8) & 0xf;
-  if ((flags >> 12) & 0xff) t.ldg_ctas_per_sm = (flags >> 12) & 0xff;
-  const int unroll = (t.ldg_unroll == 2 || t.ldg_unroll == 8) ? t.ldg_unroll : 4;
-  a.piece = (uint32_t)(kLdgThreads * unroll * vec);
+  const SliceCfg c = slice_cfg(src, dst, a.E, flags);
+  a.piece = (uint32_t)(kLdgThreads * c.unroll * c.vec);
   a.ppp = (a.pair_bytes + a.piece - 1) / a.piece;
   a.total_items = (uint64_t)n * a.T * a.ppp;
-  const uint64_t cap = (uint64_t)sm_count(src->device) * (uint64_t)std::max(1, t.ldg_ctas_per_sm);
+  const uint64_t cap = (uint64_t)sm_count(src->device) * (uint64_t)c.ctas_per_sm;
   const int grid = (int)std::max<uint64_t>(1, std::min<uint64_t>(a.total_items, cap));
   cudaError_t e;
-  switch (vec) {
-    case 16: e = launch_heads_v<int4>(a, grid, unroll, s); break;
-    case 8: e = launch_heads_v<uint2>(a, grid, unroll, s); break;
-    case 4: e = launch_heads_v<uint32_t>(a, grid, unroll, s); break;
-    default: e = launch_heads_v<uint8_t>(a, grid, unroll, s); break;
+  switch (c.vec) {
+    case 16: e = launch_heads_v<int4>(a, grid, c.unroll, s); break;
+    case 8: e = launch_heads_v<uint2>(a, grid, c.unroll, s); break;
+    case 4: e = launch_heads_v<uint32_t>(a, grid, c.unroll, s); break;
+    default: e = launch_heads_v<uint8_t>(a, grid, c.unroll, s); break;
   }
   if (e != cudaSuccess) {
     set_error("head-slice migrate launch failed: %s", cudaGetErrorString(e));
+    return KVB_ERR_CUDA;
+  }
+  count_launch();
+  return KVB_OK;
+}
+
+int launch_migrate_tokens(const kvb_pool* src, const kvb_pool* dst, const kvb_token_segment_t* segs_dev, int64_t n,
+                          int32_t max_n, int src_head0, int dst_head0, int n_heads, cudaStream_t s, int flags) {
+  if (n == 0) return KVB_OK;
+  const kvb_kv_geometry_t& gs = src->geom;
+  const kvb_kv_geometry_t& gd = dst->geom;
+  TokenArgs a{};
+  a.src_t = src->d_tensor_ptrs;
+  a.dst_t = dst->d_tensor_ptrs;
+  a.segs = segs_dev;
+  a.src_stride = src->stride_bytes;
+  a.dst_stride = dst->stride_bytes;
+  a.T = (uint32_t)src->num_tensors;
+  a.P = (uint32_t)gs.planes;
+  a.E = (uint32_t)gs.head_bytes;
+  a.Bs = (uint32_t)gs.tokens;
+  a.Bd = (uint32_t)gd.tokens;
+  a.Hs = (uint32_t)gs.heads;
+  a.Hd = (uint32_t)gd.heads;
+  a.hs0 = (uint32_t)src_head0;
+  a.hd0 = (uint32_t)dst_head0;
+  a.nh = (uint32_t)n_heads;
+  a.src_hnd = gs.layout == KVB_KV_LAYOUT_HND;
+  a.dst_hnd = gd.layout == KVB_KV_LAYOUT_HND;
+  a.run_kind = gs.layout != gd.layout ? 2 : (a.src_hnd ? 1 : 0);
+  a.tok_bytes = a.nh * a.E;
+  const SliceCfg c = slice_cfg(src, dst, a.E, flags);
+  a.piece = (uint32_t)(kLdgThreads * c.unroll * c.vec);
+  const uint32_t max_bytes = a.P * (uint32_t)max_n * a.tok_bytes;
+  a.ppp = (max_bytes + a.piece - 1) / a.piece;
+  a.total_items = (uint64_t)n * a.T * a.ppp;
+  const uint64_t cap = (uint64_t)sm_count(src->device) * (uint64_t)c.ctas_per_sm;
+  const int grid = (int)std::max<uint64_t>(1, std::min<uint64_t>(a.total_items, cap));
+  cudaError_t e;
+  switch (c.vec) {
+    case 16: e = launch_tokens_v<int4>(a, grid, c.unroll, s); break;
+    case 8: e = launch_tokens_v<uint2>(a, grid, c.unroll, s); break;
+    case 4: e = launch_tokens_v<uint32_t>(a, grid, c.unroll, s); break;
+    default: e = launch_tokens_v<uint8_t>(a, grid, c.unroll, s); break;
+  }
+  if (e != cudaSuccess) {
+    set_error("token-segment migrate launch failed: %s", cudaGetErrorString(e));
     return KVB_ERR_CUDA;
   }
   count_launch();

@@ -109,7 +109,8 @@ struct kvb_pool {
   // held by a host-id call from taking its slot until it has recorded the slot's event: calls from several host
   // threads must neither share a slot nor let the ring come round to a slot before its release is recorded
   std::mutex ids_mu;
-  // how each fragment holds its KV heads (kvb_pool_set_geometry); kvb_migrate_heads refuses pools without one
+  // how each fragment holds its KV heads (kvb_pool_set_geometry); kvb_migrate_heads and kvb_migrate_tokens refuse pools
+  // without one
   bool has_geom = false;
   kvb_kv_geometry_t geom{};
 };
@@ -127,6 +128,10 @@ int launch_migrate(const kvb_pool* src, const kvb_pool* dst, const int64_t* src_
 int launch_migrate_heads(const kvb_pool* src, const kvb_pool* dst, const int64_t* src_ids_dev,
                          const int64_t* dst_ids_dev, int64_t n, int src_head0, int dst_head0, int n_heads,
                          cudaStream_t s, int flags);
+// token segments segs_dev[0, n) of src -> dst with heads [src_head0, +n_heads) -> [dst_head0, +n_heads) (arguments
+// already checked; whole-block calls are routed to launch_migrate_heads by the caller); max_n: largest n_tokens
+int launch_migrate_tokens(const kvb_pool* src, const kvb_pool* dst, const kvb_token_segment_t* segs_dev, int64_t n,
+                          int32_t max_n, int src_head0, int dst_head0, int n_heads, cudaStream_t s, int flags);
 // copies ids into a free scratch slot and enqueues the H2D on s; after launching the kernel that reads *out_dev the
 // caller records *done_ev on s (release of the slot).  The caller holds pool->ids_mu from before this call until that
 // record.

@@ -3,6 +3,7 @@
 #include <sched.h>
 #include <sys/mman.h>
 
+#include <algorithm>
 #include <cstdarg>
 #include <cstdlib>
 #include <cstring>
@@ -576,6 +577,84 @@ int kvb_migrate_heads(kvb_pool_t* src, kvb_pool_t* dst, const int64_t* src_ids, 
     rc = upload_ids(src, both.data(), 2 * n, s, &d, &done);
     if (rc) return rc;
     rc = launch_migrate_heads(src, dst, d, d + n, n, src_head0, dst_head0, n_heads, s, flags);
+    cudaEventRecord(done, s);
+    return rc;
+  });
+}
+
+int kvb_migrate_tokens(kvb_pool_t* src, kvb_pool_t* dst, const kvb_token_segment_t* segs, int64_t n_segs,
+                       int32_t src_head0, int32_t dst_head0, int32_t n_heads, void* stream, int flags) {
+  static_assert(sizeof(kvb_token_segment_t) == 4 * sizeof(int64_t), "a segment travels as 4 id words");
+  return kvb::guarded([&]() -> int {
+    KVB_REQUIRE(src && dst, "pool is NULL");
+    KVB_REQUIRE(n_segs >= 0, "negative segment count");
+    KVB_REQUIRE(src->has_geom && dst->has_geom, "migrate_tokens: the %s pool has no KV geometry",
+                src->has_geom ? "destination" : "source");
+    const kvb_kv_geometry_t &gs = src->geom, &gd = dst->geom;
+    KVB_REQUIRE(src->num_tensors == dst->num_tensors && gs.planes == gd.planes && gs.head_bytes == gd.head_bytes,
+                "migrate_tokens: pools differ in shape (T %d vs %d, planes %d vs %d, head_bytes %d vs %d)",
+                src->num_tensors, dst->num_tensors, gs.planes, gd.planes, gs.head_bytes, gd.head_bytes);
+    KVB_REQUIRE(n_heads >= 1 && src_head0 >= 0 && dst_head0 >= 0 && (int64_t)src_head0 + n_heads <= gs.heads &&
+                    (int64_t)dst_head0 + n_heads <= gd.heads,
+                "migrate_tokens: heads [%d, +%d) -> [%d, +%d) out of range (source holds %d, destination %d)",
+                src_head0, n_heads, dst_head0, n_heads, gs.heads, gd.heads);
+    KVB_REQUIRE(dst->device == src->device,
+                "migrate_tokens: describe the destination pool on the source device (peer/IPC pointers)");
+    if (n_segs == 0) return KVB_OK;
+    KVB_REQUIRE(segs, "segments NULL");
+    int32_t max_n = 0;
+    bool whole = true;  // every segment covers a whole block on both sides
+    for (int64_t i = 0; i < n_segs; ++i) {
+      const kvb_token_segment_t& g = segs[i];
+      KVB_REQUIRE(g.n_tokens >= 1 && g.src_tok0 >= 0 && g.dst_tok0 >= 0 &&
+                      (int64_t)g.src_tok0 + g.n_tokens <= gs.tokens && (int64_t)g.dst_tok0 + g.n_tokens <= gd.tokens,
+                  "migrate_tokens: segment %lld tokens [%d, +%d) -> [%d, +%d) out of range (blocks of %d and %d tokens)",
+                  (long long)i, g.src_tok0, g.n_tokens, g.dst_tok0, g.n_tokens, gs.tokens, gd.tokens);
+      KVB_REQUIRE(g.src_block >= 0 && g.src_block < src->num_blocks && g.dst_block >= 0 &&
+                      g.dst_block < dst->num_blocks,
+                  "migrate_tokens: segment %lld blocks %lld -> %lld out of range [0,%lld) -> [0,%lld)", (long long)i,
+                  (long long)g.src_block, (long long)g.dst_block, (long long)src->num_blocks,
+                  (long long)dst->num_blocks);
+      max_n = std::max(max_n, g.n_tokens);
+      whole = whole && g.src_tok0 == 0 && g.dst_tok0 == 0 && g.n_tokens == gs.tokens && g.n_tokens == gd.tokens;
+    }
+    {  // no destination token is written twice: sorted by (block, first token), each range ends before the next starts
+      std::vector<int64_t> order(n_segs);
+      for (int64_t i = 0; i < n_segs; ++i) order[i] = i;
+      std::sort(order.begin(), order.end(), [&](int64_t a, int64_t b) {
+        return segs[a].dst_block != segs[b].dst_block ? segs[a].dst_block < segs[b].dst_block
+                                                      : segs[a].dst_tok0 < segs[b].dst_tok0;
+      });
+      for (int64_t k = 1; k < n_segs; ++k) {
+        const kvb_token_segment_t &a = segs[order[k - 1]], &b = segs[order[k]];
+        KVB_REQUIRE(a.dst_block != b.dst_block || a.dst_tok0 + a.n_tokens <= b.dst_tok0,
+                    "migrate_tokens: segments %lld and %lld overlap in destination block %lld",
+                    (long long)order[k - 1], (long long)order[k], (long long)b.dst_block);
+      }
+    }
+    DeviceGuard g(src->device);
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    const int64_t* d = nullptr;
+    cudaEvent_t done = nullptr;
+    int rc;
+    if (whole) {  // whole blocks on both sides: exactly kvb_migrate_heads on the two id lists
+      std::vector<int64_t> both(2 * n_segs);
+      for (int64_t i = 0; i < n_segs; ++i) {
+        both[i] = segs[i].src_block;
+        both[n_segs + i] = segs[i].dst_block;
+      }
+      std::lock_guard<std::mutex> lk(src->ids_mu);
+      rc = upload_ids(src, both.data(), 2 * n_segs, s, &d, &done);
+      if (rc) return rc;
+      rc = launch_migrate_heads(src, dst, d, d + n_segs, n_segs, src_head0, dst_head0, n_heads, s, flags);
+      cudaEventRecord(done, s);
+      return rc;
+    }
+    std::lock_guard<std::mutex> lk(src->ids_mu);  // the segments travel through the id ring as 4 words each
+    rc = upload_ids(src, reinterpret_cast<const int64_t*>(segs), 4 * n_segs, s, &d, &done);
+    if (rc) return rc;
+    rc = launch_migrate_tokens(src, dst, reinterpret_cast<const kvb_token_segment_t*>(d), n_segs, max_n, src_head0,
+                               dst_head0, n_heads, s, flags);
     cudaEventRecord(done, s);
     return rc;
   });

@@ -83,5 +83,37 @@ def migrate_heads(src: KVPool, dst: KVPool, src_ids: Sequence[int], dst_ids: Seq
                                         int(dst_head0), int(n_heads), _stream_ptr(stream), flags))
 
 
+_SEGMENT = np.dtype([("src_block", "<i8"), ("dst_block", "<i8"), ("src_tok0", "<i4"), ("dst_tok0", "<i4"),
+                     ("n_tokens", "<i4"), ("pad", "<i4")])  # kvb_token_segment_t
+
+
+def migrate_tokens(src: KVPool, dst: KVPool, segments, src_head0: int = 0, dst_head0: int = 0, n_heads=None,
+                   stream=None, flags: int = 0) -> None:
+    """Token segments between pools of different block sizes or at offsets inside a block (kvb.h section 5).
+    ``segments`` is an (n, 5) integer array of rows [src_block, src_tok0, dst_block, dst_tok0, n_tokens]: tokens
+    [src_tok0, +n_tokens) of source block src_block, heads [src_head0, +n_heads), go to tokens [dst_tok0, +n_tokens) of
+    destination block dst_block, heads [dst_head0, +n_heads); nothing else of the destination is written.
+    partition.token_segments plans the segments of a request.  n_heads=None means all heads and needs both pools to
+    hold the same number."""
+    seg = np.asarray(segments, dtype=np.int64)
+    if seg.size == 0:
+        seg = seg.reshape(0, 5)
+    if seg.ndim != 2 or seg.shape[1] != 5:
+        raise ValueError(f"segments must be an (n, 5) array, not {seg.shape}")
+    if n_heads is None:
+        gs, gd = src.geometry, dst.geometry
+        if gs is None or gd is None or gs.heads != gd.heads:
+            raise ValueError("n_heads=None needs both pools to carry a geometry with the same number of heads")
+        n_heads = gs.heads
+    lim = np.iinfo(np.int32)
+    if seg.size and (seg[:, [1, 3, 4]].min() < lim.min or seg[:, [1, 3, 4]].max() > lim.max):
+        raise ValueError("token offsets and counts must fit in 32 bits")
+    rec = np.zeros(seg.shape[0], dtype=_SEGMENT)
+    rec["src_block"], rec["src_tok0"], rec["dst_block"], rec["dst_tok0"], rec["n_tokens"] = seg.T
+    check(_lib.load().kvb_migrate_tokens(src.handle, dst.handle, rec.ctypes.data_as(C.POINTER(_lib.TokenSegment)),
+                                         rec.size, int(src_head0), int(dst_head0), int(n_heads), _stream_ptr(stream),
+                                         flags))
+
+
 def enable_peer_access(device: int, peer: int) -> None:
     check(_lib.load().kvb_enable_peer_access(device, peer))

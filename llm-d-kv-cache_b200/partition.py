@@ -73,6 +73,30 @@ def tp_head_transfers(num_kv_heads: int, src_tp: int, dst_tp: int, mla: bool = F
     return out
 
 
+def token_segments(src_ids, src_block_size: int, dst_ids, dst_block_size: int, n_tokens: int, src_start: int = 0,
+                   dst_start: int = 0) -> np.ndarray:
+    """Segments for migrate.migrate_tokens: token u < n_tokens of the transfer is at position src_start + u of the
+    source request (block table src_ids, blocks of src_block_size tokens) and goes to position dst_start + u of the
+    destination request.  Returns the maximal segments, an (n, 5) int64 array of [src_block, src_tok0, dst_block,
+    dst_tok0, n_tokens], cut wherever either side crosses a block boundary.  All TP ranks of an instance share one block
+    table, so one list serves every call of a tp_head_transfers plan."""
+    Bs, Bd, n = int(src_block_size), int(dst_block_size), int(n_tokens)
+    if Bs < 1 or Bd < 1 or n < 0 or src_start < 0 or dst_start < 0:
+        raise ValueError("block sizes must be >= 1, the token count and starts >= 0")
+    src_ids, dst_ids = np.asarray(src_ids, dtype=np.int64).reshape(-1), np.asarray(dst_ids, dtype=np.int64).reshape(-1)
+    if n and (src_ids.size * Bs < src_start + n or dst_ids.size * Bd < dst_start + n):
+        raise ValueError(f"{src_ids.size} source / {dst_ids.size} destination block ids do not cover tokens "
+                         f"[{src_start}, +{n}) / [{dst_start}, +{n})")
+    out, u = [], 0
+    while u < n:
+        sb, so = divmod(src_start + u, Bs)
+        db, do = divmod(dst_start + u, Bd)
+        k = min(Bs - so, Bd - do, n - u)
+        out.append((src_ids[sb], so, dst_ids[db], do, k))
+        u += k
+    return np.array(out, dtype=np.int64).reshape(-1, 5)
+
+
 def exchange_objects(obj, dist=None) -> list:
     """all_gather of one picklable object per rank (pool descriptors, checksums)."""
     if dist is None or not dist.is_initialized() or dist.get_world_size() == 1:
